@@ -25,6 +25,13 @@ constexpr int BLOCK_M = 128;
 constexpr int CONSUMER_THREADS = 256;                 // two warpgroups
 constexpr int PRODUCER_WARP = CONSUMER_THREADS / 32;
 constexpr int NUM_THREADS = CONSUMER_THREADS + 128;     // + the producer warpgroup
+constexpr int SCRATCH_BYTES = (CONSUMER_THREADS / 32) * 2048;   // the consumer warps' epilogue scratch
+
+// ring stages of `stage_bytes` that fit next to the fixed parts of shared memory (bias vectors, barriers, scratch)
+constexpr int ring_stages(int stage_bytes, int bias_floats) {
+  const int n = (227 * 1024 - (1024 /*align slack*/ + bias_floats * 4 + 2 * 8 * 8 + SCRATCH_BYTES)) / stage_bytes;
+  return n > 8 ? 8 : n;
+}
 
 // NPL = operand planes staged per k-block: 2 (hi + lo, three products) or 1 (hi only, one product: 11-bit (f16) /
 // 8-bit (bf16) operand mantissas, the arithmetic of a plain half-precision tensor-core GEMM with fp32 accumulation).
@@ -34,8 +41,10 @@ struct Cfg {
   static constexpr int W_BYTES = BLOCK_N * BLOCK_K * 2;
   // One pipeline stage holds GROUP consecutive k-blocks (64 K-elements worth): with narrow channel counts a k-block
   // is a single conv tap of 16 or 32 channels, and one barrier round trip per tap is what bounds the small-channel
-  // vocoder stages.  hi and lo planes of an operand arrive in ONE TMA box (plane dimension = 2).
-  static constexpr int GROUP = BLOCK_K >= 64 ? 1 : 64 / BLOCK_K;
+  // vocoder stages.  hi and lo planes of an operand arrive in ONE TMA box (plane dimension = 2).  The WaveNet GEMMs
+  // (GATE, RES_SKIP) take BLOCK_K 32 only where a 64-wide ring would have 2 stages (see pick_cfg), and then keep one
+  // k-block per stage: the point is a deeper ring, not fewer barrier round trips.
+  static constexpr int GROUP = BLOCK_K >= 64 || EPI == FD_EPI_GATE || EPI == FD_EPI_RES_SKIP ? 1 : 64 / BLOCK_K;
   static constexpr int SUB_BYTES = NPL * (A_BYTES + W_BYTES);           // multiple of 1024 for every instantiation
   static constexpr int STAGE_BYTES = GROUP * SUB_BYTES;
   static constexpr int TX_BYTES = SUB_BYTES;                            // per k-block
@@ -44,10 +53,7 @@ struct Cfg {
   static constexpr uint32_t SBO = 8 * SWIZZLE_BYTES;
   static constexpr int WG_A_BYTES = 64 * SWIZZLE_BYTES;                  // one warpgroup's 64 rows of a plane
   static constexpr int BIAS_FLOATS = (EPI == FD_EPI_GATE ? 3 : 1) * BLOCK_N;
-  static constexpr int SCRATCH_BYTES = (CONSUMER_THREADS / 32) * 2048;
-  static constexpr int FIXED_BYTES = 1024 /*align slack*/ + BIAS_FLOATS * 4 + 2 * 8 * 8 + SCRATCH_BYTES;
-  static constexpr int RAW_STAGES = (227 * 1024 - FIXED_BYTES) / STAGE_BYTES;
-  static constexpr int NUM_STAGES = RAW_STAGES > 8 ? 8 : RAW_STAGES;
+  static constexpr int NUM_STAGES = ring_stages(STAGE_BYTES, BIAS_FLOATS);
   static constexpr int SMEM_BYTES = 1024 /*align slack*/ + NUM_STAGES * STAGE_BYTES + BIAS_FLOATS * 4 +
                                     2 * NUM_STAGES * 8 + SCRATCH_BYTES;
   static_assert(NUM_STAGES >= 2, "pipeline needs at least two stages");
@@ -648,10 +654,20 @@ void pick_cfg(const FdTapGemm& p, int* bn, int* bk) {
   }
   const int k = all64 ? 64 : all32 ? 32 : all16 ? 16 : 0;
   if (k == 0) return;
+  // GATE / RES_SKIP (the WaveNet GEMMs): where a ring of 64-wide k-blocks holds only 2 stages (three products at
+  // BLOCK_N 256: 96 KB per stage), only one stage is ever refilled while the other is consumed.  BLOCK_K 32 halves the
+  // stage and doubles the ring; the k16 order of the wgmma calls, and so every output bit, stays the same.  Measured
+  // at the sampler shape (B=32, T=4000, C=512, H100 SXM at a 400 W power limit): GATE 3.76 -> 3.17 ms, RES_SKIP
+  // 1.38 -> 1.28 ms per launch.  Single-product mode already has 4 stages of 48 KB at BLOCK_K 64, and went 1.34 ->
+  // 1.42 ms (GATE) at BLOCK_K 32, so the switch is made only where the 64-wide ring is 2 deep.
+  const int npl = p.single ? 1 : 2;
+  auto wavenet_bk = [&](int n) {
+    return ring_stages(npl * (BLOCK_M + n) * 64 * 2, (p.epi == FD_EPI_GATE ? 3 : 1) * n) < 3 ? 32 : 64;
+  };
   if (p.epi == FD_EPI_GATE || p.epi == FD_EPI_MAG) {
     const int n = p.gate_tile;
     if ((n != 256 && n != 128) || p.n_total % n != 0 || k != 64) return;
-    *bn = n; *bk = 64;
+    *bn = n; *bk = p.epi == FD_EPI_GATE ? wavenet_bk(n) : 64;
     return;
   }
   int n = 256;
@@ -664,7 +680,7 @@ void pick_cfg(const FdTapGemm& p, int* bn, int* bk) {
     // GEMM is 314 tiles of 256 columns = 3 waves for 2.12 waves of work) was tried against 128-column tiles for LINEAR /
     // GATE_BWD whenever the quantised time came out > 5 % better: same-box A/B of the training step 12.87 / 12.81 -> 12.81 /
     // 12.80 ms (one product), 19.84 / 20.07 -> 19.87 / 19.66 ms (three products) -- noise; left out.
-    *bn = n; *bk = 64;
+    *bn = n; *bk = p.epi == FD_EPI_RES_SKIP ? wavenet_bk(n) : 64;
   } else if (k == 32) {
     if (p.epi != FD_EPI_LINEAR || n < 32) return;   // (GATE_BWD: BLOCK_K 64 only)
     *bn = n > 64 ? 64 : n; *bk = 32;
@@ -701,6 +717,15 @@ int fd_tapgemm_tc_launch(const FdTapGemm& p, cudaStream_t stream) {
     if (p.epi == FD_EPI_GATE_BWD) return launch_cfg<64, 64, FD_EPI_GATE_BWD>(p, stream);
     if (p.epi == FD_EPI_RES_SKIP) return launch_cfg<64, 64, FD_EPI_RES_SKIP>(p, stream);
     return launch_cfg<64, 64, FD_EPI_LINEAR>(p, stream);
+  }
+  if (p.epi == FD_EPI_GATE || p.epi == FD_EPI_RES_SKIP) {
+    // pick_cfg takes BLOCK_K 32 for these only at BLOCK_N 256 with three products
+    FD_REQUIRE(bk == 32 && bn == 256 && !p.single, "tapgemm(tc): no BLOCK_K=%d instantiation of epi=%d", bk, p.epi);
+    if (p.epi == FD_EPI_GATE)
+      return p.prec == FD_F16 ? launch_inst<256, 32, FD_EPI_GATE, FD_F16, 2>(p, stream)
+                              : launch_inst<256, 32, FD_EPI_GATE, FD_BF16, 2>(p, stream);
+    return p.prec == FD_F16 ? launch_inst<256, 32, FD_EPI_RES_SKIP, FD_F16, 2>(p, stream)
+                            : launch_inst<256, 32, FD_EPI_RES_SKIP, FD_BF16, 2>(p, stream);
   }
   if (bk == 32) {
     FD_REQUIRE(p.epi == FD_EPI_LINEAR, "tapgemm(tc): BLOCK_K=32 only instantiated for the linear epilogue");

@@ -1,0 +1,114 @@
+"""Per-launch device time of the two WaveNet tap-GEMMs (GEMM1 = GATE, GEMM2 = RES_SKIP) at the headline sampler shape
+(B=32, T=4000, C=512, E=256, f16), with the shared-memory traffic the tiling implies.
+
+    python tools/prof_wavenet_gemm.py [--single] [--reps N]
+
+Every dilation 1, 2, 4, 8 runs `reps` middle-layer blocks through fd_wavenet_block_fwd; each tap-GEMM launch is timed
+by its own CUDA-event pair (N.prof_enable / N.prof_collect).  Bytes staged per launch come from the tiling of
+fd_tapgemm_tc.cu: 128-row position tiles x 256-column tiles x 64-wide k-blocks, NPL operand planes each; the second
+figure is what would be staged if two CTAs on adjacent position tiles shared each W box (thread-block cluster pairs with
+a TMA multicast, see DESIGN.md section 5).  --single repeats the run in single-product mode (one hi*hi product, one plane
+staged)."""
+import argparse
+import math
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+B, T, C, E = 32, 4000, 512, 256
+BLOCK_M, BLOCK_N, BLOCK_K = 128, 256, 64
+DILATIONS = (1, 2, 4, 8)
+
+
+def staged_bytes(k_total, npl):
+    """-> (bytes into shared memory per launch without multicast, with W shared by CTA pairs)."""
+    m_tiles = B * math.ceil(T / BLOCK_M)
+    tiles = m_tiles * (2 * C // BLOCK_N)
+    kb = k_total // BLOCK_K
+    a = BLOCK_M * BLOCK_K * 2 * npl
+    w = BLOCK_N * BLOCK_K * 2 * npl
+    return tiles * kb * (a + w), tiles * kb * (a + w / 2)
+
+
+def gpu_info():
+    q = "name,power.limit,clocks.max.sm"
+    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
+    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else f"nvidia-smi failed: {r.stderr}"
+
+
+def run(N, torch, single, reps):
+    dev = torch.device("cuda", 0)
+    pc = N.PREC_F16
+    mma = pc | (N.PREC_SINGLE if single else 0)
+    g = torch.Generator(device=dev).manual_seed(0)
+    x = torch.randn(B, T, C, device=dev, generator=g)
+    cond = torch.randn(B, T, E, device=dev, generator=g)
+    w1 = torch.randn(2 * C, 3 * C + E, device=dev, generator=g) * math.sqrt(2.0 / (3 * C))
+    w2 = torch.randn(2 * C, C, device=dev, generator=g) * math.sqrt(2.0 / C)
+    gb = torch.randn(3, 2 * C, device=dev, generator=g) * 0.1
+    b2 = torch.randn(2 * C, device=dev, generator=g) * 0.1
+    s1, s2 = N.pow2_scale(w1), N.pow2_scale(w2)
+    w1p, w2p = N.pack_weight(w1, pc, s1), N.pack_weight(w2, pc, s2)
+    xp, cp = N.split_nwc(x, pc), N.split_nwc(cond, pc)
+    del x, cond
+    z = torch.zeros((2, B, T, C), dtype=torch.int16, device=dev)
+    skip = torch.zeros((B, T, C), dtype=torch.float32, device=dev)
+    skp = torch.zeros((2, B, T, C), dtype=torch.int16, device=dev)
+    st = N.stream_ptr(dev)
+
+    def block(dil):
+        # flags 0: a middle layer (reads and writes the fp32 skip accumulator, updates the residual planes)
+        N.check(N.lib().fd_wavenet_block_fwd(
+            N.ptr(xp), N.ptr(cp), N.ptr(z), N.ptr(w1p), N.ptr(w2p), N.ptr(gb[0]), N.ptr(gb[1]), N.ptr(gb[2]), 0,
+            N.ptr(b2), N.ptr(skip), N.ptr(skp), 1.0, B, T, C, E, dil, 256, 1.0 / s1, 1.0 / s2, 0, mma, N.BACKEND_TC,
+            st), "fd_wavenet_block_fwd")
+
+    for dil in DILATIONS:          # warm-up: module load, tensor maps, clocks
+        for _ in range(5):
+            block(dil)
+    torch.cuda.synchronize()
+    N.prof_enable(True)
+    for dil in DILATIONS:
+        for _ in range(reps):
+            block(dil)
+    prof, overflow = N.prof_collect()
+    N.prof_enable(False)
+    assert not overflow, "per-launch event buffer overflowed: lower --reps"
+
+    npl = 1 if single else 2
+    mode = "single product (hi*hi)" if single else "three products (lo*hi + hi*lo + hi*hi)"
+    print(f"== {mode}, B={B} T={T} C={C} E={E}, dilations {DILATIONS} x {reps} blocks")
+    for name, key, k_total in (("GEMM1 gate", "gate/tc", 3 * C + E), ("GEMM2 res_skip", "res_skip/tc", C)):
+        ms_sum, n = prof[key]
+        ms = ms_sum / n
+        alg = 2.0 * B * T * (2 * C) * k_total
+        products = 1 if single else 3
+        plain, mcast = staged_bytes(k_total, npl)
+        print(f"{name:15s} {ms:7.3f} ms/launch over {n} launches ({ms_sum / 1e3:.2f} s) | "
+              f"{alg / ms / 1e9:6.1f} TFLOP/s alg, {products}x issued = "
+              f"{products * alg / ms / 1e9:6.1f} TFLOP/s | smem staged {plain / 1e9:5.2f} GB/launch "
+              f"({plain / ms / 1e9:5.2f} TB/s L2->SM), with W shared by CTA pairs {mcast / 1e9:5.2f} GB "
+              f"({mcast / ms / 1e9:5.2f} TB/s)", flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--single", action="store_true", help="also run in single-product mode")
+    ap.add_argument("--reps", type=int, default=200, help="blocks per dilation in the timed window")
+    args = ap.parse_args()
+    import torch
+    import __graft_entry__ as ge
+    ge.build()
+    from fish_diffusion_b200 import _native as N
+    assert torch.cuda.is_available(), "prof_wavenet_gemm.py needs a CUDA device"
+    print(f"gpu: {gpu_info()} (name, power limit, max SM clock)")
+    run(N, torch, False, args.reps)
+    if args.single:
+        run(N, torch, True, args.reps)
+
+
+if __name__ == "__main__":
+    main()
