@@ -379,9 +379,13 @@ def tc_supported_linear(n_total: int, k_seg: int, num_seg: int) -> bool:
 def gemm_cl(src0, C0, w_planes, n_total, k_total, B, T, segs, *, src1=None, C1=0, strides0=None, strides1=None,
             w_kshift=0, w_bstride_k=0, bias=None, bias_per_item=False, addend=None, res_f32=None, res_planes=None, res_scale=1.0,
             row_mask=None, out_f32=None, out_planes=None, w_inv_scale=1.0, post_scale=1.0, planes_scale=1.0,
-            act=ACT_NONE, act_slope=0.0, out_accum=False, prec=PREC_F16, backend=BACKEND_TC):
+            act=ACT_NONE, act_slope=0.0, out_accum=False, prec=PREC_F16, backend=BACKEND_TC, gate_y=None, gate_tile=0,
+            gate_dil=0, gate_cs=None, gate_cs_edge=None, gate_cs_scale=1.0):
     """General linear tap-GEMM (fd_gemm_cl_fwd).  segs = [(src_index, shift, c_off, k_len), ...];
-    stridesX = (row_stride, batch_stride, plane_stride) in elements or None for the canonical [2][B][T][C]."""
+    stridesX = (row_stride, batch_stride, plane_stride) in elements or None for the canonical [2][B][T][C].
+    gate_y (planes [2,B,T,2n_total] of packed pre-activations) turns the epilogue into the gate backward: out_planes
+    gets dy in packed order, gate_cs [B,2n_total] / gate_cs_edge [2,B,2n_total] (fp32, optional) accumulate
+    gate_cs_scale * its column sums over all steps / the first and last gate_dil steps."""
     d = GemmDesc()
     d.src[0], d.src_C[0] = ptr(src0), C0
     d.src[1], d.src_C[1] = ptr(src1), C1
@@ -398,6 +402,8 @@ def gemm_cl(src0, C0, w_planes, n_total, k_total, B, T, segs, *, src1=None, C1=0
     d.planes_scale, d.act_slope = planes_scale, act_slope
     d.out_accum, d.act, d.prec, d.backend = int(out_accum), act, prec, backend
     d.bias_bstride = n_total if bias_per_item else 0
+    d.gate_y, d.gate_cs, d.gate_cs_edge = ptr(gate_y), ptr(gate_cs), ptr(gate_cs_edge)
+    d.gate_cs_scale, d.gate_tile, d.gate_dil = gate_cs_scale, gate_tile, gate_dil
     check(lib().fd_gemm_cl_fwd(ctypes.byref(d), stream_ptr(src0.device)), "fd_gemm_cl_fwd")
 
 

@@ -705,9 +705,11 @@ int fd_tapgemm_tc_supported(const FdTapGemm& p) {
 int fd_tapgemm_tc_launch(const FdTapGemm& p, cudaStream_t stream) {
   int bn, bk;
   pick_cfg(p, &bn, &bk);
-  FD_REQUIRE((long long)p.B * p.T * p.n_total < (1ll << 32),
-             "tapgemm(tc): B*T*n_total = %lld exceeds the 32-bit element offsets of the epilogue",
-             (long long)p.B * p.T * p.n_total);
+  // the epilogues index their outputs with 32-bit element offsets; GATE_BWD's are into the 2C-wide dy / y planes
+  const long long width = p.epi == FD_EPI_GATE_BWD ? 2ll * p.n_total : p.n_total;
+  FD_REQUIRE((long long)p.B * p.T * width < (1ll << 32),
+             "tapgemm(tc): B*T*%lld = %lld exceeds the 32-bit element offsets of the epilogue", width,
+             (long long)p.B * p.T * width);
   FD_REQUIRE(bn != 0 && fd_tapgemm_tc_supported(p),
              "tapgemm(tc): no tensor-core instantiation for n_total=%d k_total=%d epi=%d", p.n_total, p.k_total,
              p.epi);
