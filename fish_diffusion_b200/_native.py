@@ -20,7 +20,7 @@ PREC_F16, PREC_BF16 = 0, 1
 PREC_SINGLE = 0x10   # or-ed into the prec of GEMM calls: one product over the hi planes
 BACKEND_TC, BACKEND_SIMT = 0, 1
 ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 class NativeError(RuntimeError):
@@ -42,9 +42,8 @@ class ConvDesc(ctypes.Structure):
 class GemmDesc(ctypes.Structure):
     """struct fd_gemm_desc (include/fishdiff_b200.h)."""
     _fields_ = [
-        ("src", c_void_p * 2), ("src_C", c_int * 2), ("src_rs", c_longlong * 2), ("src_bs", c_longlong * 2),
-        ("src_ps", c_longlong * 2), ("w", c_void_p), ("n_total", c_int), ("k_total", c_int), ("w_kshift", c_int),
-        ("w_bstride_k", c_longlong), ("B", c_int), ("T", c_int), ("num_seg", c_int), ("seg_src", c_int * 16),
+        ("src", c_void_p * 2), ("src_C", c_int * 2), ("w", c_void_p), ("n_total", c_int), ("k_total", c_int),
+        ("w_kshift", c_int), ("B", c_int), ("T", c_int), ("num_seg", c_int), ("seg_src", c_int * 16),
         ("seg_shift", c_int * 16), ("seg_coff", c_int * 16), ("seg_klen", c_int * 16),
         ("bias", c_void_p), ("addend", c_void_p), ("res_f32", c_void_p), ("res_planes", c_void_p),
         ("row_mask", c_void_p), ("out_f32", c_void_p), ("out_planes", c_void_p),
@@ -108,6 +107,7 @@ class WgradDesc(ctypes.Structure):
         ("num_col_seg", c_int), ("col_seg_src", c_int * 8), ("col_seg_shift", c_int * 8), ("col_seg_coff", c_int * 8),
         ("col_seg_width", c_int * 8),
         ("B", c_int), ("T", c_int), ("splits", c_int), ("part", c_void_p), ("acc_scale", c_float), ("prec", c_int),
+        ("backend", c_int),
     ]
 
 
@@ -120,8 +120,6 @@ _SIGS = {
     "fd_wavenet_block_fwd_train": (c_int, [c_void_p] * 10 + [c_int, c_void_p, c_void_p, c_void_p, c_float] +
                                    [c_int] * 6 + [c_float, c_float, c_int, c_int, c_int, c_void_p]),
     "fd_wavenet_gate_bias_from_d": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_void_p]),
-    "fd_fold_transpose": (c_int, [c_void_p] * 4 + [c_int, c_void_p] + [c_int] * 5 + [c_float, c_int, c_int, c_int,
-                                                                                   c_int, c_int, c_void_p]),
     "fd_gate_bwd": (c_int, [c_void_p] * 3 + [c_longlong, c_int, c_int, c_int, c_void_p]),
     "fd_relu_bwd": (c_int, [c_void_p] * 3 + [c_longlong, c_float, c_int, c_void_p]),
     "fd_lrelu_bwd": (c_int, [c_void_p] * 5 + [c_longlong, c_float, c_float, c_int, c_void_p]),
@@ -376,23 +374,19 @@ def tc_supported_linear(n_total: int, k_seg: int, num_seg: int) -> bool:
     return bool(lib().fd_tc_supported_linear(n_total, k_seg, num_seg))
 
 
-def gemm_cl(src0, C0, w_planes, n_total, k_total, B, T, segs, *, src1=None, C1=0, strides0=None, strides1=None,
-            w_kshift=0, w_bstride_k=0, bias=None, bias_per_item=False, addend=None, res_f32=None, res_planes=None, res_scale=1.0,
-            row_mask=None, out_f32=None, out_planes=None, w_inv_scale=1.0, post_scale=1.0, planes_scale=1.0,
+def gemm_cl(src0, C0, w_planes, n_total, k_total, B, T, segs, *, src1=None, C1=0, w_kshift=0, bias=None,
+            bias_per_item=False, addend=None, res_f32=None, res_planes=None, res_scale=1.0, row_mask=None, out_f32=None, out_planes=None, w_inv_scale=1.0, post_scale=1.0, planes_scale=1.0,
             act=ACT_NONE, act_slope=0.0, out_accum=False, prec=PREC_F16, backend=BACKEND_TC, gate_y=None, gate_tile=0,
             gate_dil=0, gate_cs=None, gate_cs_edge=None, gate_cs_scale=1.0):
-    """General linear tap-GEMM (fd_gemm_cl_fwd).  segs = [(src_index, shift, c_off, k_len), ...];
-    stridesX = (row_stride, batch_stride, plane_stride) in elements or None for the canonical [2][B][T][C].
+    """General linear tap-GEMM (fd_gemm_cl_fwd).  segs = [(src_index, shift, c_off, k_len), ...]; w_kshift offsets the
+    K coordinate of W (a column block of a wider W).
     gate_y (planes [2,B,T,2n_total] of packed pre-activations) turns the epilogue into the gate backward: out_planes
     gets dy in packed order, gate_cs [B,2n_total] / gate_cs_edge [2,B,2n_total] (fp32, optional) accumulate
     gate_cs_scale * its column sums over all steps / the first and last gate_dil steps."""
     d = GemmDesc()
     d.src[0], d.src_C[0] = ptr(src0), C0
     d.src[1], d.src_C[1] = ptr(src1), C1
-    for i, st in enumerate((strides0, strides1)):
-        if st is not None:
-            d.src_rs[i], d.src_bs[i], d.src_ps[i] = st
-    d.w, d.n_total, d.k_total, d.w_kshift, d.w_bstride_k = ptr(w_planes), n_total, k_total, int(w_kshift), int(w_bstride_k)
+    d.w, d.n_total, d.k_total, d.w_kshift = ptr(w_planes), n_total, k_total, int(w_kshift)
     d.B, d.T, d.num_seg = B, T, len(segs)
     for j, (si, sh, co, kl) in enumerate(segs):
         d.seg_src[j], d.seg_shift[j], d.seg_coff[j], d.seg_klen[j] = si, sh, co, kl
@@ -408,26 +402,30 @@ def gemm_cl(src0, C0, w_planes, n_total, k_total, B, T, segs, *, src1=None, C1=0
 
 
 def wgrad_supported(row_segs, col_segs) -> bool:
-    """Shapes the direct (MN-major wgmma) weight-gradient kernel takes: every segment a multiple of 64 channels."""
+    """Shapes the tensor-core (MN-major wgmma) weight-gradient kernel takes: every segment a multiple of 64 channels.
+    The SIMT twin takes multiples of 8."""
     return (1 <= len(row_segs) <= 2 and 1 <= len(col_segs) <= 8 and all(w % 64 == 0 and w > 0 for *_, w in row_segs)
             and all(w % 64 == 0 and w > 0 for *_, w in col_segs))
 
 
 def wgrad_splits(R, Cc, B, T):
-    """Item splits of a direct weight-gradient GEMM (see wgrad_cl): enough work units for ~2 waves of the 132 SMs of an
-    H100, at most one partial per item, and one accumulation run kept to <= ~2048 time steps."""
+    """Item splits of a weight-gradient GEMM (see wgrad_cl): enough work units for ~2 waves of the 132 SMs of an H100 at
+    the tensor-core tiling, at most one partial per item, and one accumulation run kept to <= ~2048 time steps (the
+    tensor cores' fp32 accumulation truncates: long runs put relative noise of the order of 1e-4 on the conditioner /
+    input-projection weight gradients)."""
     bn = 256 if Cc % 256 == 0 else 128 if Cc % 128 == 0 else 64
-    tiles = ((R + 127) // 128) * (Cc // bn)
+    tiles = ((R + 127) // 128) * -(-Cc // bn)
     splits = max(1, min(B, -(-264 // tiles)))
     splits = max(splits, -(-B // max(1, 2048 // T)))
     ips = -(-B // splits)
     return -(-B // ips)
 
 
-def wgrad_cl(row_srcs, col_srcs, row_segs, col_segs, B, T, *, scale=1.0, prec=PREC_F16, splits=None, out=None):
+def wgrad_cl(row_srcs, col_srcs, row_segs, col_segs, B, T, *, scale=1.0, prec=PREC_F16, splits=None, out=None,
+             backend=BACKEND_TC):
     """sum_{b,t} ROW[b,t,r] * COL[b,t+shift,c] * scale -> fp32 [R, Cc]  (fd_wgrad_cl + fd_reduce_batch).
     row_srcs / col_srcs: lists of 1..2 plane tensors [2,B,T,C]; row_segs = [(src, c_off, width)],
-    col_segs = [(src, shift, c_off, width)]."""
+    col_segs = [(src, shift, c_off, width)]; widths are multiples of 64 on BACKEND_TC (wgrad_supported), 8 on SIMT."""
     import torch
     d = WgradDesc()
     for i, t in enumerate(row_srcs):
@@ -444,18 +442,12 @@ def wgrad_cl(row_srcs, col_srcs, row_segs, col_segs, B, T, *, scale=1.0, prec=PR
     for j, (si, sh, co, w) in enumerate(col_segs):
         d.col_seg_src[j], d.col_seg_shift[j], d.col_seg_coff[j], d.col_seg_width[j] = si, sh, co, w
         Cc += w
-    if splits is None:      # enough work units for ~2 waves of the 132 SMs, at most one partial per item
-        bn = 256 if Cc % 256 == 0 else 128 if Cc % 128 == 0 else 64
-        tiles = ((R + 127) // 128) * (Cc // bn)
-        splits = max(1, min(B, -(-264 // tiles)))
-        # tensor-core fp32 accumulation truncates: keep one accumulation run to <= ~2048 time steps (long runs put
-        # relative noise of the order of 1e-4 on the conditioner / input-projection weight gradients)
-        splits = max(splits, -(-B // max(1, 2048 // T)))
-    ips = -(-B // splits)
-    splits = -(-B // ips)
+    if splits is None:
+        splits = wgrad_splits(R, Cc, B, T)
+    splits = -(-B // -(-B // splits))       # the kernel refuses empty splits
     dev = row_srcs[0].device
     part = torch.empty((splits, R, Cc), dtype=torch.float32, device=dev)
-    d.B, d.T, d.splits, d.part, d.acc_scale, d.prec = B, T, splits, ptr(part), 1.0, prec
+    d.B, d.T, d.splits, d.part, d.acc_scale, d.prec, d.backend = B, T, splits, ptr(part), 1.0, prec, backend
     st = stream_ptr(dev)
     check(lib().fd_wgrad_cl(ctypes.byref(d), st), "fd_wgrad_cl")
     if out is None:

@@ -320,15 +320,14 @@ int fd_gemm_cl_fwd(const fd_gemm_desc* d, void* stream) {
     FD_REQUIRE(d->seg_src[j] == 0 || d->seg_src[j] == 1, "fd_gemm_cl_fwd: segment %d has bad source", j);
     p.seg[j] = FdSeg{d->seg_src[j], d->seg_shift[j], d->seg_coff[j], d->seg_klen[j]};
   }
-  for (int i = 0; i < 2; ++i) {
-    if (d->src[i] == nullptr) continue;
-    set_src(p, i, d->src[i], d->src_C[i]);
-    if (d->src_rs[i] != 0) p.src_rs[i] = d->src_rs[i];
-    if (d->src_bs[i] != 0) p.src_bs[i] = d->src_bs[i];
-    if (d->src_ps[i] != 0) p.src_ps[i] = d->src_ps[i];
-  }
+  for (int i = 0; i < 2; ++i)
+    if (d->src[i] != nullptr) set_src(p, i, d->src[i], d->src_C[i]);
   FD_REQUIRE(p.src[0] != nullptr, "fd_gemm_cl_fwd: src[0] is null");
-  p.w = d->w; p.acc_scale = d->w_inv_scale; p.w_kshift = d->w_kshift; p.w_bstride_k = d->w_bstride_k;
+  int k_sum = 0;
+  for (int j = 0; j < d->num_seg; ++j) k_sum += d->seg_klen[j];
+  FD_REQUIRE(d->w_kshift >= 0 && d->w_kshift + k_sum <= d->k_total,
+             "fd_gemm_cl_fwd: w_kshift=%d + K=%d exceeds the W row pitch k_total=%d", d->w_kshift, k_sum, d->k_total);
+  p.w = d->w; p.acc_scale = d->w_inv_scale; p.w_kshift = d->w_kshift;
   p.epi = FD_EPI_LINEAR;
   p.bias = d->bias; p.bias_bstride = d->bias_bstride;
   if (d->gate_y != nullptr) {

@@ -55,10 +55,9 @@ struct FdTapGemm {
   long long src_rs[2], src_bs[2], src_ps[2];
   const uint16_t* w;        // split planes [2][n_total][k_total]
   float acc_scale;          // accumulators are multiplied by this (undoes power-of-two weight prescale)
-  // W-operand K offsets (weight-gradient GEMMs, where "W" is a transposed activation tensor [rows][B*Tp]):
-  // the K coordinate of the W operand is  koff(seg) + k0 + w_kshift + b * w_bstride_k
+  // K offset of the W operand (a multiple of 8): the K coordinate of W is  koff(seg) + k0 + w_kshift, which selects a
+  // column block of a wider W (the skip half of W2^T in the last layer's dz GEMM)
   int w_kshift;
-  long long w_bstride_k;
   int epi;
 
   // ---- FD_EPI_LINEAR:  y = acc*acc_scale + bias[n] + addend[b,t,n] + res[b,t,n];  y *= post_scale
@@ -117,6 +116,24 @@ struct FdTapGemm {
   float* cs;                // [B][2C] or null
   float* cs_edge;           // [2][B][2C] or null
   float cs_scale;
+};
+
+// Weight-gradient GEMM (fd_wgrad_cl), resolved by the entry point for both back ends:
+//   part[s][r][c] = acc_scale * sum_{b in split s} sum_t ROW[b, t, r] * COL[b, t + shift(c), c]
+// rows / columns are concatenated segments; segment g covers rows [row_start[g], row_start[g] + row_width[g]) and reads
+// channels from row_coff[g] on of source row_src[g] (likewise for columns, plus a time shift).
+#define FD_WGRAD_MAX_COL_SEG 8
+struct FdWgradK {
+  int B, T, R, Cc;
+  int splits, items_per_split;
+  int m_tiles, n_tiles;     // tile counts of the tensor-core kernel
+  int num_row_seg, num_col_seg;
+  int row_src[2], row_coff[2], row_start[2], row_width[2];
+  int col_src[FD_WGRAD_MAX_COL_SEG], col_shift[FD_WGRAD_MAX_COL_SEG], col_coff[FD_WGRAD_MAX_COL_SEG],
+      col_start[FD_WGRAD_MAX_COL_SEG], col_width[FD_WGRAD_MAX_COL_SEG];
+  int row_C[2], col_C[2];
+  float* part;
+  float acc_scale;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -451,3 +468,5 @@ void fd_set_error(const char* fmt, ...);
 int fd_tapgemm_simt_launch(const FdTapGemm& p, cudaStream_t stream);
 int fd_tapgemm_tc_launch(const FdTapGemm& p, cudaStream_t stream);
 int fd_tapgemm_tc_supported(const FdTapGemm& p);
+int fd_wgrad_simt_launch(const FdWgradK& p, const uint16_t* const* row_ptr, const uint16_t* const* col_ptr, int prec,
+                         cudaStream_t stream);

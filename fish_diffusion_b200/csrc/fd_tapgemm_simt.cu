@@ -1,7 +1,8 @@
-// SIMT fp32 twin of the tap-GEMM (same operands, same packed weights, same epilogues as the
-// wgmma kernel in fd_tapgemm_tc.cu).  It exists (a) as the device-side check of the tensor-core
-// kernel, (b) for shapes the tensor-core instantiations do not cover.  It is plain CUDA-core FFMA
-// over (hi+lo) recombined operands, i.e. fp32 arithmetic on 22-bit (f16 planes) inputs.
+// SIMT fp32 twins of the tap-GEMM (same operands, same packed weights, same epilogues as the
+// wgmma kernel in fd_tapgemm_tc.cu) and of the weight-gradient GEMM (fd_wgrad_tc.cu).  They exist
+// (a) as the device-side check of the tensor-core kernels, (b) for shapes the tensor-core
+// instantiations do not cover.  They are plain CUDA-core FFMA over (hi+lo) recombined operands,
+// i.e. fp32 arithmetic on 22-bit (f16 planes) inputs.
 #include "fd_common.cuh"
 
 namespace {
@@ -78,21 +79,9 @@ __global__ void __launch_bounds__(256) fd_tapgemm_simt_kernel(const FdTapGemm p)
         const int kk = k0 + kh * 8;
         float v[8];
         if (n < p.n_total && kk < sg.k_len) {
-          const long long kw = (long long)koff + kk + p.w_kshift + (long long)b * p.w_bstride_k;
-          if (p.w_kshift == 0 && p.w_bstride_k == 0) {
-            if (p.single) fd_load_hi8(p.w, (size_t)n * p.k_total + kw, v, p.prec);
-            else fd_load_planes<8>(p.w, w_plane, (size_t)n * p.k_total + kw, v, p.prec);
-          } else {   // weight-gradient mode: unaligned / out-of-range K coordinates read as zero (like the TMA box)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const long long ki = kw + i;
-              v[i] = (ki >= 0 && ki < p.k_total)
-                         ? (p.single ? fd_h2f(p.w[(size_t)n * p.k_total + ki], p.prec)
-                                     : fd_combine(p.w[(size_t)n * p.k_total + ki],
-                                                  p.w[w_plane + (size_t)n * p.k_total + ki], p.prec))
-                         : 0.f;
-            }
-          }
+          const size_t off = (size_t)n * p.k_total + koff + kk + p.w_kshift;
+          if (p.single) fd_load_hi8(p.w, off, v, p.prec);
+          else fd_load_planes<8>(p.w, w_plane, off, v, p.prec);
         } else {
 #pragma unroll
           for (int i = 0; i < 8; ++i) v[i] = 0.f;
@@ -171,11 +160,97 @@ int launch_run(const FdTapGemm& p, cudaStream_t stream) {
   return 0;
 }
 
+// ---- weight gradient (fd_wgrad_cl): one CTA per (split, WG_R-row tile, WG_C-column tile) loops over the items of its
+//      split and their time steps, WG_T steps at a time; both operands are staged [t][channel] in shared memory
+constexpr int WG_R = 64, WG_C = 64, WG_T = 16;
+
+__global__ void __launch_bounds__(256) fd_wgrad_simt_kernel(const FdWgradK p, const uint16_t* row0,
+                                                            const uint16_t* row1, const uint16_t* col0,
+                                                            const uint16_t* col1, int prec, int single) {
+  static_assert(WG_R == WG_C, "rows and columns share the staging code");
+  __shared__ __align__(16) float Rs[WG_T][WG_R + 4];
+  __shared__ __align__(16) float Cs[WG_T][WG_C + 4];
+  const int tid = threadIdx.x;
+  const int s = blockIdx.z, r0 = blockIdx.y * WG_R, c0 = blockIdx.x * WG_C;
+
+  // staging: threads [0,128) load rows, [128,256) columns; each thread one 8-channel group at one time step of a block.
+  // Segment widths and starts are multiples of 8, so a group lies in one segment (or past the last one: zeros).
+  const bool is_col = tid >= 128;
+  const int grp = tid % 8, tl = (tid % 128) / 8;
+  const int i = (is_col ? c0 : r0) + grp * 8;
+  const uint16_t* src = nullptr;
+  int C = 0, ch = 0, shift = 0;
+  if (!is_col) {
+    for (int g = 0; g < p.num_row_seg; ++g)
+      if (i >= p.row_start[g] && i < p.row_start[g] + p.row_width[g]) {
+        src = p.row_src[g] == 0 ? row0 : row1;
+        C = p.row_C[p.row_src[g]]; ch = p.row_coff[g] + (i - p.row_start[g]);
+      }
+  } else {
+    for (int g = 0; g < p.num_col_seg; ++g)
+      if (i >= p.col_start[g] && i < p.col_start[g] + p.col_width[g]) {
+        src = p.col_src[g] == 0 ? col0 : col1;
+        C = p.col_C[p.col_src[g]]; ch = p.col_coff[g] + (i - p.col_start[g]); shift = p.col_shift[g];
+      }
+  }
+  const size_t plane = (size_t)p.B * p.T * C;
+  float* const dst = is_col ? &Cs[tl][grp * 8] : &Rs[tl][grp * 8];
+
+  const int tx = tid % 16, ty = tid / 16;      // this thread's outputs: rows r0 + 4 ty .. +4, columns c0 + 4 tx .. +4
+  float acc[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[r][c] = 0.f;
+
+  const int b_end = min(p.B, (s + 1) * p.items_per_split);
+  for (int b = s * p.items_per_split; b < b_end; ++b) {
+    for (int t0 = 0; t0 < p.T; t0 += WG_T) {
+      const int t = t0 + tl, ts = t + shift;   // a column segment's tap shift reads zero outside [0,T)
+      float v[8];
+      if (src != nullptr && t < p.T && ts >= 0 && ts < p.T) {
+        const size_t off = ((size_t)b * p.T + ts) * C + ch;
+        if (single) fd_load_hi8(src, off, v, prec);
+        else fd_load_planes<8>(src, plane, off, v, prec);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = 0.f;
+      }
+      *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+      *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < WG_T; ++k) {
+        const float4 a = *reinterpret_cast<const float4*>(&Rs[k][ty * 4]);
+        const float4 c = *reinterpret_cast<const float4*>(&Cs[k][tx * 4]);
+        const float av[4] = {a.x, a.y, a.z, a.w}, cv[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int cc = 0; cc < 4; ++cc) acc[r][cc] = fmaf(av[r], cv[cc], acc[r][cc]);
+      }
+      __syncthreads();
+    }
+  }
+
+  const int col = c0 + tx * 4;                 // Cc is a multiple of 8: a 4-column group is all in or all out
+  if (col >= p.Cc) return;
+  float* const out = p.part + (size_t)s * p.R * p.Cc;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int row = r0 + ty * 4 + r;
+    if (row < p.R)
+      *reinterpret_cast<float4*>(out + (size_t)row * p.Cc + col) = make_float4(
+          acc[r][0] * p.acc_scale, acc[r][1] * p.acc_scale, acc[r][2] * p.acc_scale, acc[r][3] * p.acc_scale);
+  }
+}
+
 }  // namespace
 
 int fd_tapgemm_simt_launch(const FdTapGemm& p, cudaStream_t stream) {
   FD_REQUIRE(p.n_total % 4 == 0, "tapgemm(simt): n_total=%d must be a multiple of 4", p.n_total);
-  FD_REQUIRE(p.k_total % 8 == 0, "tapgemm(simt): k_total=%d must be a multiple of 8", p.k_total);
+  FD_REQUIRE(p.k_total % 8 == 0 && p.w_kshift % 8 == 0,
+             "tapgemm(simt): k_total=%d and w_kshift=%d must be multiples of 8", p.k_total, p.w_kshift);
   for (int s = 0; s < p.num_seg; ++s) {
     FD_REQUIRE(p.seg[s].k_len % 8 == 0 && p.seg[s].c_off % 8 == 0 && p.src_rs[p.seg[s].src] % 8 == 0 &&
                    p.src_bs[p.seg[s].src] % 8 == 0 && p.src_ps[p.seg[s].src] % 8 == 0,
@@ -193,4 +268,13 @@ int fd_tapgemm_simt_launch(const FdTapGemm& p, cudaStream_t stream) {
   }
   if (p.n_total >= 96) return launch_run<64>(p, stream);
   return launch_run<16>(p, stream);
+}
+
+int fd_wgrad_simt_launch(const FdWgradK& p, const uint16_t* const* row_ptr, const uint16_t* const* col_ptr, int prec,
+                         cudaStream_t stream) {
+  dim3 grid((p.Cc + WG_C - 1) / WG_C, (p.R + WG_R - 1) / WG_R, p.splits);
+  fd_wgrad_simt_kernel<<<grid, 256, 0, stream>>>(p, row_ptr[0], row_ptr[1], col_ptr[0], col_ptr[1], prec & 0xF,
+                                                 (prec & FD_SINGLE) != 0);
+  FD_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }

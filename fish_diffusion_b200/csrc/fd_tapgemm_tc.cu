@@ -118,7 +118,7 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
             const CUtensorMap* tm = sg.src == 0 ? &tm_src0 : &tm_src1;
             uint8_t* sub = st + g * C::SUB_BYTES;
             tma_load_4d(sub, tm, &full_bar[stage], sg.c_off + k0, t0 + sg.shift, b, 0);          // hi + lo planes
-            const int kw = koff + k0 + p.w_kshift + (int)(b * p.w_bstride_k);
+            const int kw = koff + k0 + p.w_kshift;
             tma_load_3d(sub + NPL * C::A_BYTES, &tm_w, &full_bar[stage], kw, n0, 0);               // hi + lo planes
             k0 += BLOCK_K;
             if (k0 >= sg.k_len) { koff += sg.k_len; k0 = 0; ++s; }

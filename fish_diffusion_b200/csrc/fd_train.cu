@@ -1,65 +1,13 @@
-// Memory-bound kernels of the WaveNet training step (backward pass).  The six gradient GEMMs per residual block
-// are tap-GEMM launches (fd_tapgemm_*.cu): data gradients use transposed packed weights with mirrored tap shifts,
-// weight gradients use the same kernel with "rows" = output channels and K = time, fed by the folded transposes
-// produced here (wavenet.py:106-120 differentiated by hand; checked against the reference's autograd in the tests).
+// Memory-bound kernels of the WaveNet training step (backward pass), and fd_wavenet_block_bwd, which issues the whole
+// backward of one residual block on either back end (wavenet.py:106-120 differentiated by hand; checked against the
+// reference's autograd in the tests).  Data gradients are tap-GEMM launches (fd_tapgemm_*.cu) on transposed packed
+// weights with mirrored tap shifts; weight gradients are fd_wgrad_cl launches that read both operands straight from the
+// channels-last planes, with time as the contraction axis.
 #include <cstring>
 #include "fd_common.cuh"
 #include "fd_host.h"
 
 namespace {
-
-// planes [2][B][T][C] (+ optional per-(item, channel) addend d) -> planes [2][C][B][Tp], item b's T samples start at
-// column PAD of its Tp-wide span, everything else is zero.  `mode`: 0 plain, 1 z = sigmoid(g)*tanh(f) computed from a
-// packed pre-activation tensor (C = residual channels, source has 2C packed columns), 2 relu-mask (src is a fp32
-// gradient [B][T][C], `aux` planes give the forward activation; value = grad * (act > 0)).
-template <int MODE>
-__global__ void k_fold_transpose(const uint16_t* __restrict__ src, const float* __restrict__ src_f32,
-                                 const uint16_t* __restrict__ aux, const float* __restrict__ addvec, int add_bstride,
-                                 uint16_t* __restrict__ dst, int B, int T, int C, int Tp, int pad, float scale,
-                                 int gate_tile, int prec, int dst_rows, int dst_row0) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z;
-  const int c0 = blockIdx.y * 32, t0 = blockIdx.x * 32;   // t0 indexes the padded axis
-  const size_t splane = MODE == 1 ? (size_t)B * T * 2 * C : (size_t)B * T * C;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int tp = t0 + i, c = c0 + threadIdx.x;
-    const int t = tp - pad;
-    float v = 0.f;
-    if (t >= 0 && t < T && c < C) {
-      const size_t row = (size_t)b * T + t;
-      if (MODE == 0) {
-        const size_t off = row * C + c;
-        v = fd_combine(src[off], src[splane + off], prec);
-        if (addvec != nullptr) v += addvec[(size_t)b * add_bstride + c];
-      } else if (MODE == 1) {
-        const int half = gate_tile / 2;
-        const int ng = (c / half) * gate_tile + (c % half);
-        const size_t off = row * 2 * C + ng;
-        const float g = fd_combine(src[off], src[splane + off], prec);
-        const float f = fd_combine(src[off + half], src[splane + off + half], prec);
-        v = fd_sigmoid(g) * fd_tanh(f);
-      } else {
-        const size_t off = row * C + c;
-        const float a = fd_combine(aux[off], aux[splane + off], prec);
-        v = a > 0.f ? src_f32[off] : 0.f;
-      }
-      v *= scale;
-    }
-    tile[i][threadIdx.x] = v;
-  }
-  __syncthreads();
-  const size_t dplane = (size_t)dst_rows * B * Tp;      // the destination may be a taller stacked operand
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, tp = t0 + threadIdx.x;
-    if (c < C && tp < Tp) {
-      uint16_t hi, lo;
-      fd_split(tile[threadIdx.x][i], prec, hi, lo);
-      const size_t off = ((size_t)(dst_row0 + c) * B + b) * Tp + tp;
-      dst[off] = hi;
-      dst[dplane + off] = lo;
-    }
-  }
-}
 
 // dz (fp32 [rows][C]) and packed pre-activations y (planes [2][rows][2C]) -> dy planes [2][rows][2C] (packed order):
 //   z = sigmoid(g) tanh(f);  dg = dz * tanh(f) * sg (1 - sg);  df = dz * sg * (1 - tanh(f)^2)
@@ -185,30 +133,6 @@ inline int grid1d(long long work, int block = 256, int cap = 132 * 16) {
 
 extern "C" {
 
-int fd_fold_transpose(const uint16_t* src_planes, const float* src_f32, const uint16_t* aux_planes, const float* addvec,
-                      int add_bstride, uint16_t* dst, int B, int T, int C, int Tp, int pad, float scale, int mode,
-                      int gate_tile, int prec, int dst_rows, int dst_row0, void* stream) {
-  FD_DEVICE_GUARD();
-  FD_REQUIRE(Tp >= T + pad && pad >= 0, "fd_fold_transpose: Tp=%d too small for T=%d pad=%d", Tp, T, pad);
-  if (dst_rows <= 0) { dst_rows = C; dst_row0 = 0; }
-  FD_REQUIRE(dst_row0 >= 0 && dst_row0 + C <= dst_rows, "fd_fold_transpose: rows [%d,%d) outside the %d-row destination",
-             dst_row0, dst_row0 + C, dst_rows);
-  FD_REQUIRE(mode >= 0 && mode <= 2, "fd_fold_transpose: bad mode %d", mode);
-  dim3 grid((Tp + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (mode == 0)
-    k_fold_transpose<0><<<grid, block, 0, st>>>(src_planes, nullptr, nullptr, addvec, add_bstride, dst, B, T, C, Tp, pad,
-                                                scale, gate_tile, prec, dst_rows, dst_row0);
-  else if (mode == 1)
-    k_fold_transpose<1><<<grid, block, 0, st>>>(src_planes, nullptr, nullptr, nullptr, 0, dst, B, T, C, Tp, pad, scale,
-                                                gate_tile, prec, dst_rows, dst_row0);
-  else
-    k_fold_transpose<2><<<grid, block, 0, st>>>(nullptr, src_f32, aux_planes, nullptr, 0, dst, B, T, C, Tp, pad, scale,
-                                                gate_tile, prec, dst_rows, dst_row0);
-  FD_LAUNCHED();
-  return 0;
-}
-
 int fd_gate_bwd(const float* dz, const uint16_t* y_planes, uint16_t* dy_planes, long long rows, int C, int gate_tile,
                 int prec, void* stream) {
   FD_DEVICE_GUARD();
@@ -274,20 +198,29 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
   FD_DEVICE_GUARD();
   FD_REQUIRE(d != nullptr, "fd_wavenet_block_bwd: null descriptor");
   const int B = d->B, T = d->T, C = d->C, E = d->E, dil = d->dilation;
-  FD_REQUIRE(B > 0 && T > 0 && C % 64 == 0 && E % 64 == 0 && dil > 0, "fd_wavenet_block_bwd: bad shape B=%d T=%d C=%d E=%d", B, T, C, E);
+  const bool tc = d->backend == FD_BACKEND_TC;
+  const int unit = tc ? 64 : 8;    // the tensor-core weight gradient takes 64-channel segments, its SIMT twin 8
+  FD_REQUIRE(B > 0 && T > 0 && C % unit == 0 && E % unit == 0 && dil > 0,
+             "fd_wavenet_block_bwd: bad shape B=%d T=%d C=%d E=%d (backend %d)", B, T, C, E, d->backend);
   const float inv_sqrt2 = 0.70710678118654752440f;
-  const long long rows = (long long)B * T;
+  const int edge = dil < T ? dil : T;
   int rc;
-  // ---- dy = gate backward of dz = [dx_next | d_skip] . W2, fused into the GEMM's epilogue together with the column
-  //      sums of dy (K offset C selects the skip half of W2^T when there is no residual gradient)
+  // ---- dy = gate backward of dz = [dx_next | d_skip] . W2 and the column sums of dy (K offset C selects the skip half
+  //      of W2^T when there is no residual gradient).  Tensor cores fuse the gate backward and the sums into the GEMM's
+  //      epilogue; the SIMT twin writes dz and runs them as separate kernels.
   {
     fd_gemm_desc g;
     memset(&g, 0, sizeof(g));
     g.w = d->w2t; g.n_total = C; g.k_total = 2 * C; g.B = B; g.T = T;
     g.w_inv_scale = d->w2t_inv; g.res_scale = 1.f; g.post_scale = 1.f; g.planes_scale = 1.f;
-    g.out_planes = d->dy; g.prec = d->prec; g.backend = d->backend;
-    g.gate_y = d->y_planes; g.gate_tile = d->gate_tile; g.gate_dil = dil < T ? dil : T;
-    g.gate_cs = d->cs_dy; g.gate_cs_edge = d->cs_edge; g.gate_cs_scale = d->inv_S;
+    g.prec = d->prec; g.backend = d->backend;
+    if (tc) {
+      g.out_planes = d->dy;
+      g.gate_y = d->y_planes; g.gate_tile = d->gate_tile; g.gate_dil = edge;
+      g.gate_cs = d->cs_dy; g.gate_cs_edge = d->cs_edge; g.gate_cs_scale = d->inv_S;
+    } else {
+      g.out_f32 = d->dz;
+    }
     if (d->dx_next == nullptr) {
       g.src[0] = d->dskip; g.src_C[0] = C; g.num_seg = 1; g.w_kshift = C;
       g.seg_src[0] = 0; g.seg_shift[0] = 0; g.seg_coff[0] = 0; g.seg_klen[0] = C;
@@ -297,6 +230,15 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
     }
     rc = fd_gemm_cl_fwd(&g, stream);
     if (rc) return rc;
+    if (!tc) {
+      const int prec = d->prec & 0xF;
+      rc = fd_gate_bwd(d->dz, d->y_planes, d->dy, (long long)B * T, C, d->gate_tile, prec, stream);
+      if (rc) return rc;
+      rc = fd_colsum(d->dy, nullptr, d->cs_dy, B, T, 2 * C, d->inv_S, prec, stream);
+      if (rc) return rc;
+      rc = fd_colsum_edges(d->dy, d->cs_edge, B, T, 2 * C, edge, d->inv_S, prec, stream);
+      if (rc) return rc;
+    }
   }
   // ---- gw2 = [dx_next ; d_skip]^T . z
   {
@@ -304,6 +246,7 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
     memset(&w, 0, sizeof(w));
     w.col_src[0] = d->z_planes; w.col_C[0] = C; w.num_col_seg = 1; w.col_seg_width[0] = C;
     w.B = B; w.T = T; w.splits = d->splits2; w.part = d->part2; w.acc_scale = 1.f; w.prec = d->prec;
+    w.backend = d->backend;
     float* out = d->gw2;
     int R = 2 * C;
     if (d->dx_next == nullptr) {
@@ -329,6 +272,7 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
     for (int j = 0; j < 3; ++j) { w.col_seg_src[j] = 0; w.col_seg_shift[j] = sh[j]; w.col_seg_width[j] = C; }
     w.col_seg_src[3] = 1; w.col_seg_width[3] = E;
     w.B = B; w.T = T; w.splits = d->splits1; w.part = d->part1; w.acc_scale = 1.f; w.prec = d->prec;
+    w.backend = d->backend;
     rc = fd_wgrad_cl(&w, stream);
     if (rc) return rc;
     rc = fd_reduce_batch(d->part1, d->gw1, d->splits1, (long long)2 * C * (3 * C + E), d->inv_S, stream);

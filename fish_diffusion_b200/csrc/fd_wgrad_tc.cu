@@ -1,13 +1,14 @@
-// Weight-gradient GEMM on wgmma straight from channels-last split planes (sm_90a).
+// Weight-gradient GEMM on wgmma straight from channels-last split planes (sm_90a), and the fd_wgrad_cl entry point,
+// which also serves the SIMT twin (fd_tapgemm_simt.cu).
 //
 //   part[s][r][c] = acc_scale * sum_{b in split s} sum_t  ROW[b, t, r] * COL[b, t + shift(c), c]
 //
 // Time is the contraction axis, and in channels-last storage it is the SLOW axis of both operands.  Instead of
-// transposing the activations (the fd_fold_transpose passes of the K-major path), both operands are fed to the tensor
-// core as MN-major shared-memory tiles: a TMA box of [64 time steps][64 channels] with the 128-byte swizzle is exactly
-// one MN-major SW128 atom column (64 channels contiguous = one 128-byte row per time step, 8 rows per swizzle atom), so
-// the wgmma instructions just set the transpose flags of both operands.  The conv-tap shift of a column segment is a TMA
-// row coordinate (zero fill outside [0,T) = the conv zero padding), exactly as in the forward kernel.
+// transposing the activations, both operands are fed to the tensor core as MN-major shared-memory tiles: a TMA box
+// of [64 time steps][64 channels] with the 128-byte swizzle is exactly one MN-major SW128 atom column (64 channels
+// contiguous = one 128-byte row per time step, 8 rows per swizzle atom), so the wgmma instructions just set the
+// transpose flags of both operands.  The conv-tap shift of a column segment is a TMA row coordinate (zero fill
+// outside [0,T) = the conv zero padding), exactly as in the forward kernel.
 //
 // Work unit = (split s, 128-row tile, BLOCK_N-column tile); a unit accumulates over its items and all time blocks in
 // registers and stores one fp32 partial; fd_reduce_batch sums the `splits` partials.  Warp roles and the pipeline are
@@ -26,20 +27,6 @@ constexpr int WG_CONSUMER_THREADS = 256;
 constexpr int WG_PRODUCER_WARP = WG_CONSUMER_THREADS / 32;
 constexpr int WG_THREADS = WG_CONSUMER_THREADS + 128;     // + the producer warpgroup
 constexpr int WG_BOX_BYTES = 64 * 64 * 2;      // one plane of one [64 t][64 ch] box
-constexpr int WG_MAX_COL_SEG = 8;
-
-struct FdWgradK {
-  int B, T, R, Cc;
-  int splits, items_per_split;
-  int m_tiles, n_tiles;
-  int num_row_seg, num_col_seg;
-  int row_src[2], row_coff[2], row_start[2], row_width[2];
-  int col_src[WG_MAX_COL_SEG], col_shift[WG_MAX_COL_SEG], col_coff[WG_MAX_COL_SEG], col_start[WG_MAX_COL_SEG],
-      col_width[WG_MAX_COL_SEG];
-  int row_C[2], col_C[2];
-  float* part;
-  float acc_scale;
-};
 
 template <int BLOCK_N, int NPL>
 struct WgCfg {
@@ -267,14 +254,20 @@ int launch_wg_prec(const FdWgradK& p, int prec, const uint16_t* const* row_ptr, 
 
 }  // namespace
 
+// Segment validation and row / column resolution are shared by both back ends; only the width rule differs.
 extern "C" int fd_wgrad_cl(const fd_wgrad_desc* d, void* stream) {
   FD_DEVICE_GUARD();
   FD_REQUIRE(d != nullptr, "fd_wgrad_cl: null descriptor");
+  FD_REQUIRE(d->backend == FD_BACKEND_TC || d->backend == FD_BACKEND_SIMT, "fd_wgrad_cl: unknown backend %d",
+             d->backend);
   FD_REQUIRE(d->B > 0 && d->T > 0 && d->splits > 0 && d->splits <= d->B, "fd_wgrad_cl: bad B=%d T=%d splits=%d", d->B,
              d->T, d->splits);
-  FD_REQUIRE(d->num_row_seg >= 1 && d->num_row_seg <= 2 && d->num_col_seg >= 1 && d->num_col_seg <= WG_MAX_COL_SEG,
+  FD_REQUIRE(d->num_row_seg >= 1 && d->num_row_seg <= 2 && d->num_col_seg >= 1 &&
+                 d->num_col_seg <= FD_WGRAD_MAX_COL_SEG,
              "fd_wgrad_cl: segment counts out of range (%d rows, %d cols)", d->num_row_seg, d->num_col_seg);
   FD_REQUIRE(d->part != nullptr && d->row_src[0] != nullptr && d->col_src[0] != nullptr, "fd_wgrad_cl: null pointer");
+  // tensor cores: whole 64-channel TMA boxes; SIMT twin: 8-channel vector loads
+  const int unit = d->backend == FD_BACKEND_TC ? 64 : 8;
   FdWgradK p;
   memset(&p, 0, sizeof(p));
   p.B = d->B; p.T = d->T; p.splits = d->splits; p.items_per_split = (d->B + d->splits - 1) / d->splits;
@@ -288,20 +281,20 @@ extern "C" int fd_wgrad_cl(const fd_wgrad_desc* d, void* stream) {
   for (int g = 0; g < d->num_row_seg; ++g) {
     const int src = d->row_seg_src[g];
     FD_REQUIRE((src == 0 || src == 1) && d->row_src[src] != nullptr, "fd_wgrad_cl: row segment %d has no source", g);
-    FD_REQUIRE(d->row_seg_width[g] > 0 && d->row_seg_width[g] % 64 == 0 && d->row_seg_coff[g] % 8 == 0 &&
-                   d->row_seg_coff[g] + d->row_seg_width[g] <= d->row_C[src],
-               "fd_wgrad_cl: row segment %d (coff %d width %d) must be a multiple of 64 inside the source", g,
-               d->row_seg_coff[g], d->row_seg_width[g]);
+    FD_REQUIRE(d->row_seg_width[g] > 0 && d->row_seg_width[g] % unit == 0 && d->row_seg_coff[g] >= 0 &&
+                   d->row_seg_coff[g] % 8 == 0 && d->row_seg_coff[g] + d->row_seg_width[g] <= d->row_C[src],
+               "fd_wgrad_cl: row segment %d (coff %d width %d) must be a multiple of %d inside the source", g,
+               d->row_seg_coff[g], d->row_seg_width[g], unit);
     p.row_src[g] = src; p.row_coff[g] = d->row_seg_coff[g]; p.row_start[g] = R; p.row_width[g] = d->row_seg_width[g];
     R += d->row_seg_width[g];
   }
   for (int g = 0; g < d->num_col_seg; ++g) {
     const int src = d->col_seg_src[g];
     FD_REQUIRE((src == 0 || src == 1) && d->col_src[src] != nullptr, "fd_wgrad_cl: column segment %d has no source", g);
-    FD_REQUIRE(d->col_seg_width[g] > 0 && d->col_seg_width[g] % 64 == 0 && d->col_seg_coff[g] % 8 == 0 &&
-                   d->col_seg_coff[g] + d->col_seg_width[g] <= d->col_C[src],
-               "fd_wgrad_cl: column segment %d (coff %d width %d) must be a multiple of 64 inside the source", g,
-               d->col_seg_coff[g], d->col_seg_width[g]);
+    FD_REQUIRE(d->col_seg_width[g] > 0 && d->col_seg_width[g] % unit == 0 && d->col_seg_coff[g] >= 0 &&
+                   d->col_seg_coff[g] % 8 == 0 && d->col_seg_coff[g] + d->col_seg_width[g] <= d->col_C[src],
+               "fd_wgrad_cl: column segment %d (coff %d width %d) must be a multiple of %d inside the source", g,
+               d->col_seg_coff[g], d->col_seg_width[g], unit);
     p.col_src[g] = src; p.col_shift[g] = d->col_seg_shift[g]; p.col_coff[g] = d->col_seg_coff[g];
     p.col_start[g] = Cc; p.col_width[g] = d->col_seg_width[g];
     Cc += d->col_seg_width[g];
@@ -309,14 +302,18 @@ extern "C" int fd_wgrad_cl(const fd_wgrad_desc* d, void* stream) {
   p.R = R; p.Cc = Cc;
   p.num_row_seg = d->num_row_seg; p.num_col_seg = d->num_col_seg;
   p.part = d->part; p.acc_scale = d->acc_scale;
-  p.m_tiles = (R + WG_BLOCK_M - 1) / WG_BLOCK_M;
-  const int bn = Cc % 256 == 0 ? 256 : Cc % 128 == 0 ? 128 : 64;
-  p.n_tiles = Cc / bn;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  if (bn == 256) rc = launch_wg_prec<256>(p, d->prec, d->row_src, d->col_src, st);
-  else if (bn == 128) rc = launch_wg_prec<128>(p, d->prec, d->row_src, d->col_src, st);
-  else rc = launch_wg_prec<64>(p, d->prec, d->row_src, d->col_src, st);
+  if (d->backend == FD_BACKEND_SIMT) {
+    rc = fd_wgrad_simt_launch(p, d->row_src, d->col_src, d->prec, st);
+  } else {
+    p.m_tiles = (R + WG_BLOCK_M - 1) / WG_BLOCK_M;
+    const int bn = Cc % 256 == 0 ? 256 : Cc % 128 == 0 ? 128 : 64;
+    p.n_tiles = Cc / bn;
+    if (bn == 256) rc = launch_wg_prec<256>(p, d->prec, d->row_src, d->col_src, st);
+    else if (bn == 128) rc = launch_wg_prec<128>(p, d->prec, d->row_src, d->col_src, st);
+    else rc = launch_wg_prec<64>(p, d->prec, d->row_src, d->col_src, st);
+  }
   if (rc == 0) fd_count_launch(1);
   return rc;
 }

@@ -3,24 +3,24 @@ built from the same tap-GEMM kernels (reference: autograd through fish_diffusion
 inside GaussianDiffusion.p_losses, diffusion.py:129-151).
 
 Per residual block the backward is 5 GEMM launches (2x the forward FLOPs), issued by ONE native call
-(fd_wavenet_block_bwd) on the tensor-core path:
+(fd_wavenet_block_bwd) on either back end:
   dz      = [dx_next/sqrt2 | d_skip] . W2                        data gradient of the output projection (K = 2C)
   dW2     = [dx_next/sqrt2 ; d_skip]^T . z                       weight gradient (K = time)
   dW1     = dy^T . [x(t-d)+d ; x(t)+d ; x(t+d)+d ; cond]         weight gradient of conv taps + conditioner, one GEMM
   dx      = sum_tap dy(t -/+ d) . W1_tap + dx_next/sqrt2         data gradient of the dilated conv (K = 6C)
   dcond  += dy . Wc
-Weight gradients read both operands straight from the channels-last planes (MN-major tensor-core operands, fd_wgrad_cl);
-the step vector d_l added to x inside the conv is a rank-one term added afterwards (_add_step_vector_term).  With
-`net.grad_sync` set (train.GradSync) every finished bucket of layers is handed to an NCCL all-reduce from inside the
-loop, overlapping the backward of the layers below.  A K-major path on folded transposes (fd_fold_transpose) remains
-for the SIMT back end and channel counts that are not multiples of 64.  The tiny step-embedding MLP / diffusion
-projections stay under torch autograd (they act on [B or 1, C] vectors); their output d enters the block through the
-gate-bias tables and its gradient is a column sum of dx.
+Weight gradients read both operands straight from the channels-last planes (fd_wgrad_cl: MN-major operands on the
+tensor cores, which take segments of 64 channels; the SIMT twin takes any multiple of 8, so it serves the SIMT back end
+and narrow channel counts); the step vector d_l added to x inside the conv is a rank-one term added afterwards
+(_add_step_vector_term).  With `net.grad_sync` set (train.GradSync) every finished bucket of layers is handed to an
+NCCL all-reduce from inside the loop, overlapping the backward of the layers below.  The tiny step-embedding MLP /
+diffusion projections stay under torch autograd (they act on [B or 1, C] vectors); their output d enters the block
+through the gate-bias tables and its gradient is a column sum of dx.
 """
 from __future__ import annotations
 
+import ctypes
 import math
-import os
 
 import torch
 
@@ -131,8 +131,6 @@ class WaveNetTrainFn(torch.autograd.Function):
         i16 = dict(dtype=torch.int16, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
         inv_sqrt2, inv_sqrtL = 1.0 / math.sqrt(2.0), 1.0 / math.sqrt(L)
-        PAD = max(pk["dil"])
-        Tp = (T + 2 * PAD + 63) // 64 * 64
         rows = B * T
         KT = 3 * C + E
 
@@ -149,25 +147,6 @@ class WaveNetTrainFn(torch.autograd.Function):
         inv_S = 1.0 / S
 
         # ---------------------------------------------------------------- helpers
-        def fold(planes, Cc, dst=None, row0=0, mode=0, scale=1.0, src_f32=None, aux=None, addvec=None, add_bstride=0,
-                 pad=None):
-            """planes [2,B,T,Cc] -> rows [row0, row0+Cc) of dst [2,R,B,Tp] (a fresh [2,Cc,B,Tp] when dst is None)"""
-            if dst is None:
-                dst = torch.empty((2, Cc, B, Tp), **i16)
-            N.check(lib.fd_fold_transpose(N.ptr(planes), N.ptr(src_f32), N.ptr(aux), N.ptr(addvec), add_bstride,
-                                          N.ptr(dst), B, T, Cc, Tp, PAD if pad is None else pad, scale, mode, gate_tile,
-                                          prec, dst.shape[1], row0, st), "fd_fold_transpose")
-            return dst
-
-        def wgrad(rowsT, R, colsT, Cc):
-            """sum_{b,t} rows[b,t,r] * cols[b,t,c] / S  -> fp32 [R, Cc]  (per-item partials, then one reduction)"""
-            part = torch.empty((B, R, Cc), **f32)
-            N.gemm_cl(rowsT, Tp, colsT, Cc, B * Tp, B, R, [(0, 0, 0, Tp)], strides0=(B * Tp, Tp, R * B * Tp),
-                      w_bstride_k=Tp, out_f32=part, prec=mma, backend=_backend_for(pref, Cc, Tp, 1))
-            out = torch.empty((R, Cc), **f32)
-            N.check(lib.fd_reduce_batch(N.ptr(part), N.ptr(out), B, R * Cc, inv_S, st), "fd_reduce_batch")
-            return out
-
         def colsum(planes=None, f32t=None, Nn=0):
             # gradients stored in planes are S-scaled; fp32 inputs are not
             out = torch.zeros((B, Nn), **f32)
@@ -179,14 +158,11 @@ class WaveNetTrainFn(torch.autograd.Function):
             N.gemm_cl(src0, C0, w, n_total, k_total, B, T, segs, w_inv_scale=w_inv, prec=mma,
                       backend=_backend_for(pref, n_total, segs[0][3], len(segs)), **kw)
 
-        # Direct weight gradients (fd_wgrad_cl): the tensor core reads both operands MN-major straight from the
-        # channels-last planes, so no transposed copies exist on this path; the K-major fold path below it serves the
-        # SIMT back end and channel counts that are not multiples of 64.
-        direct = (pref == N.BACKEND_TC and C % 64 == 0 and E % 64 == 0 and M % 64 == 0 and
-                  os.environ.get("FD_WGRAD_DIRECT", "1") != "0")
-
-        def wgrad_direct(row_srcs, row_segs, col_srcs, col_segs, out=None):
-            return N.wgrad_cl(row_srcs, col_srcs, row_segs, col_segs, B, T, scale=inv_S, prec=mma, out=out)
+        def wgrad(row_src, R, col_src, Cc):
+            """sum_{b,t} rows[b,t,r] * cols[b,t,c] / S -> fp32 [R, Cc], read straight from the channels-last planes"""
+            row_segs, col_segs = [(0, 0, R)], [(0, 0, 0, Cc)]
+            backend = N.BACKEND_TC if pref == N.BACKEND_TC and N.wgrad_supported(row_segs, col_segs) else N.BACKEND_SIMT
+            return N.wgrad_cl([row_src], [col_src], row_segs, col_segs, B, T, scale=inv_S, prec=mma, backend=backend)
 
         grads = {}
 
@@ -195,141 +171,79 @@ class WaveNetTrainFn(torch.autograd.Function):
         if sv["x_mask"] is not None:
             de = de.masked_fill(sv["x_mask"].bool()[:, :, None], 0.0)
         de_planes = N.split_nwc(de, prec, scale=S)
-        if direct:
-            grads["output_projection.w"] = wgrad_direct([de_planes], [(0, 0, M)], [sv["h_planes"]], [(0, 0, 0, C)])
-        else:
-            grads["output_projection.w"] = wgrad(fold(de_planes, M), M, fold(sv["h_planes"], C), C)   # [M, C]
+        grads["output_projection.w"] = wgrad(de_planes, M, sv["h_planes"], C)                   # [M, C]
         grads["output_projection.b"] = colsum(f32t=de, Nn=M).sum(0)
         dh_raw = torch.empty((B, T, C), **f32)
         dgrad(de_planes, M, bw["wot"], bw["wot_inv"], C, M, [(0, 0, 0, M)], out_f32=dh_raw)
         dh_planes = torch.empty((2, B, T, C), **i16)
         N.check(lib.fd_relu_bwd(N.ptr(dh_raw), N.ptr(sv["h_planes"]), N.ptr(dh_planes), rows * C, 1.0, prec, st),
                 "fd_relu_bwd")
-        if direct:
-            grads["skip_projection.w"] = wgrad_direct([dh_planes], [(0, 0, C)], [sv["s_planes"]], [(0, 0, 0, C)])
-        else:
-            grads["skip_projection.w"] = wgrad(fold(dh_planes, C), C, fold(sv["s_planes"], C), C)
+        grads["skip_projection.w"] = wgrad(dh_planes, C, sv["s_planes"], C)
         grads["skip_projection.b"] = colsum(planes=dh_planes, Nn=C).sum(0)
         dskip_planes = torch.empty((2, B, T, C), **i16)                           # d(skip_l) = ds / sqrt(L), every layer
         dgrad(dh_planes, C, bw["wst"], bw["wst_inv"], C, C, [(0, 0, 0, C)], out_planes=dskip_planes,
               planes_scale=inv_sqrtL)
         cs_skip = colsum(planes=dskip_planes, Nn=C)                              # [B, C]
-        if direct:
-            cs_dy = torch.zeros((L, B, 2 * C), **f32)                            # column sums of dy per item
-            cs_edge = torch.zeros((L, 2, B, 2 * C), **f32)                       # ... over the first / last `dil` steps
-            gw2_all = torch.empty((L, 2 * C, C), **f32)
-        else:
-            # stacked operands of the two weight-gradient GEMMs; the layer-invariant rows are written once
-            do_stack = torch.zeros((2, 2 * C, B, Tp), **i16)                     # [dx_next/sqrt2 ; d_skip]^T
-            fold(dskip_planes, C, dst=do_stack, row0=C)
-            xc_stack = torch.empty((2, KT, B, Tp), **i16)                        # [x(t-d)+d ; x(t)+d ; x(t+d)+d ; cond]^T
-            fold(sv["cond_planes"], E, dst=xc_stack, row0=3 * C)
-            dyT = torch.empty((2, 2 * C, B, Tp), **i16)
-            zT = torch.empty((2, C, B, Tp), **i16)
         d_cond = torch.zeros((B, T, E), **f32) if ctx.need_cond else None
 
         # ---------------------------------------------------------------- residual blocks, last to first
-        dx_next = None            # planes of d(x_{l+1}); None above the last layer (its residual output is unused)
-        cs_next = None            # column sums of dx_next per item
-        d_d = torch.zeros((Bs, L, C), **f32)
+        # One native call per block (fd_wavenet_block_bwd); per-layer column sums land in [L, ...] arrays and are turned
+        # into bias / step-vector gradients for all layers at once after the loop.
+        cs_dy = torch.zeros((L, B, 2 * C), **f32)                            # column sums of dy per item
+        cs_edge = torch.zeros((L, 2, B, 2 * C), **f32)                       # ... over the first / last `dil` steps
+        cs_x = torch.zeros((L + 1, B, C), **f32)                             # colsum of d(x_l); row L stays zero
+        gw1_all = torch.empty((L, 2 * C, KT), **f32)                         # packed row order, un-permuted at the end
+        gw2_all = torch.empty((L, 2 * C, C), **f32)
         dz = torch.empty((B, T, C), **f32)
         dx0 = torch.empty((B, T, C), **f32)       # fp32 copy of d(x_0), written by the layer-0 data gradient
         dy = torch.empty((2, B, T, 2 * C), **i16)
         dx_bufs = [torch.empty((2, B, T, C), **i16) for _ in range(2)]
-        gw1_all = torch.empty((L, 2 * C, KT), **f32)       # packed row order, un-permuted once at the end
-        gb1_all = torch.empty((L, 2 * C), **f32)
-        sync = getattr(net, "grad_sync", None) if direct else None     # overlapped gradient all-reduce (train.GradSync)
+        sync = getattr(net, "grad_sync", None)   # overlapped gradient all-reduce (train.GradSync)
         net._synced_in_backward = sync is not None
-        if direct:
-            # ---- one native call per block (fd_wavenet_block_bwd); per-layer column sums land in [L, ...] arrays and are
-            #      turned into bias / step-vector gradients for all layers at once after the loop
-            cs_x = torch.zeros((L + 1, B, C), **f32)                              # colsum of d(x_l); row L stays zero
-            splits1, splits2 = N.wgrad_splits(2 * C, KT, B, T), N.wgrad_splits(2 * C, C, B, T)
-            part1 = torch.empty((splits1, 2 * C, KT), **f32)
-            part2 = torch.empty((splits2, 2 * C, C), **f32)
-            bd = N.WaveNetBwdDesc()
-            bd.cond_planes, bd.dskip = N.ptr(sv["cond_planes"]), N.ptr(dskip_planes)
-            bd.d_cond, bd.dz, bd.dy = N.ptr(d_cond), N.ptr(dz), N.ptr(dy)
-            bd.part1, bd.part2, bd.splits1, bd.splits2 = N.ptr(part1), N.ptr(part2), splits1, splits2
-            bd.B, bd.T, bd.C, bd.E, bd.gate_tile = B, T, C, E, gate_tile
-            bd.inv_S, bd.prec, bd.backend = inv_S, mma, N.BACKEND_TC
-            dl_all = sv["d"].transpose(0, 1)                                       # [L,Bs,C]
-            bucket = sync.bucket_layers if sync is not None else L
-            import ctypes as _ct
-            for l in reversed(range(L)):
-                dx_l = dx_bufs[l & 1]
-                bd.x_planes, bd.y_planes, bd.z_planes = N.ptr(sv["xs"][l]), N.ptr(sv["ys"][l]), N.ptr(sv["zs"][l])
-                bd.dx_next = N.ptr(dx_next)
-                bd.w2t, bd.w1t, bd.wct = N.ptr(bw["w2t"][l]), N.ptr(bw["w1t"][l]), N.ptr(bw["wct"][l])
-                bd.w2t_inv, bd.w1t_inv, bd.wct_inv = bw["w2t_inv"][l], bw["w1t_inv"][l], bw["wct_inv"][l]
-                bd.dx_out, bd.dx_f32 = N.ptr(dx_l), N.ptr(dx0 if l == 0 else None)
-                bd.gw1, bd.gw2 = N.ptr(gw1_all[l]), N.ptr(gw2_all[l])
-                bd.cs_dy, bd.cs_edge, bd.cs_dx = N.ptr(cs_dy[l]), N.ptr(cs_edge[l]), N.ptr(cs_x[l])
-                bd.dilation = pk["dil"][l]
-                N.check(lib.fd_wavenet_block_bwd(_ct.byref(bd), st), "fd_wavenet_block_bwd")
-                dx_next = dx_l
-                if sync is not None and (l % bucket == 0):
-                    # layers [l, hi) are final: add their rank-one step-vector term (it depends on this rank's d) and
-                    # start the all-reduce of the bucket; it overlaps the backward of the layers below
-                    hi = min(L, l + bucket)
-                    _add_step_vector_term(gw1_all[l:hi], cs_dy[l:hi], cs_edge[l:hi], dl_all[l:hi], Bs, C)
-                    sync.reduce_async(gw1_all[l:hi], gw2_all[l:hi])
-            cs_next = None
-            d_d = cs_x[:L] - cs_x[1:] * inv_sqrt2                                  # [L,B,C] gradient wrt the step vectors d_l
-            d_d = d_d.transpose(0, 1) if Bs > 1 else d_d.sum(1, keepdim=True).transpose(0, 1)
-            d_d = d_d.contiguous()
-            gb2_all = torch.cat([cs_x[1:].sum(1) * inv_sqrt2, cs_skip.sum(0).expand(L, C)], dim=1)   # [L,2C]
-            for l in range(L):
-                grads[f"l{l}.b2"] = gb2_all[l]
-        # ---- K-major fold path (SIMT back end, channel counts that are not multiples of 64): conv by conv
-        for l in (reversed(range(L)) if not direct else ()):
-            dil = pk["dil"][l]
-            if dx_next is None:     # K offset C selects the skip half of W2^T (aligned: C % 8 == 0)
-                N.gemm_cl(dskip_planes, C, bw["w2t"][l], C, 2 * C, B, T, [(0, 0, 0, C)], w_kshift=C, out_f32=dz,
-                          w_inv_scale=bw["w2t_inv"][l], prec=mma, backend=_backend_for(pref, C, C, 1))
-            else:
-                N.gemm_cl(dx_next, C, bw["w2t"][l], C, 2 * C, B, T, [(0, 0, 0, C), (1, 0, 0, C)], src1=dskip_planes,
-                          C1=C, out_f32=dz, w_inv_scale=bw["w2t_inv"][l], prec=mma,
-                          backend=_backend_for(pref, C, C, 2))
-            N.check(lib.fd_gate_bwd(N.ptr(dz), N.ptr(sv["ys"][l]), N.ptr(dy), rows, C, gate_tile, prec, st), "fd_gate_bwd")
-            gb2 = torch.cat([cs_next.sum(0) * inv_sqrt2 if cs_next is not None else torch.zeros(C, **f32),
-                             cs_skip.sum(0)])
-            # ---- weight gradient of the output projection: rows [residual | skip] x z
-            fold(sv["ys"][l], C, dst=zT, mode=1)
-            if dx_next is not None:
-                fold(dx_next, C, dst=do_stack, row0=0, scale=inv_sqrt2)
-            grads[f"l{l}.w2"], grads[f"l{l}.b2"] = wgrad(do_stack, 2 * C, zT, C), gb2
-            # ---- weight gradient of the dilated conv taps + conditioner projection in one GEMM (packed layout)
-            fold(dy, 2 * C, dst=dyT)
-            addvec = sv["d"][:, l, :].contiguous()                                   # [Bs, C]
-            for j, sh in enumerate((-dil, 0, dil)):
-                fold(sv["xs"][l], C, dst=xc_stack, row0=j * C, addvec=addvec, add_bstride=C if Bs > 1 else 0,
-                     pad=PAD - sh)
-            gw1_all[l] = wgrad(dyT, 2 * C, xc_stack, KT)
-            gb1_all[l] = colsum(planes=dy, Nn=2 * C).sum(0)
-            # ---- data gradients: dx_l = conv^T(dy) + dx_next/sqrt2 ;  dcond += dy . Wc
+        splits1, splits2 = N.wgrad_splits(2 * C, KT, B, T), N.wgrad_splits(2 * C, C, B, T)
+        part1 = torch.empty((splits1, 2 * C, KT), **f32)
+        part2 = torch.empty((splits2, 2 * C, C), **f32)
+        bd = N.WaveNetBwdDesc()
+        bd.cond_planes, bd.dskip = N.ptr(sv["cond_planes"]), N.ptr(dskip_planes)
+        bd.d_cond, bd.dz, bd.dy = N.ptr(d_cond), N.ptr(dz), N.ptr(dy)
+        bd.part1, bd.part2, bd.splits1, bd.splits2 = N.ptr(part1), N.ptr(part2), splits1, splits2
+        bd.B, bd.T, bd.C, bd.E, bd.gate_tile = B, T, C, E, gate_tile
+        bd.inv_S, bd.prec = inv_S, mma
+        bd.backend = N.BACKEND_TC if pref == N.BACKEND_TC and C % 64 == 0 and E % 64 == 0 else N.BACKEND_SIMT
+        dl_all = sv["d"].transpose(0, 1)                                       # [L,Bs,C]
+        bucket = sync.bucket_layers if sync is not None else L
+        dx_next = None            # planes of d(x_{l+1}); None above the last layer (its residual output is unused)
+        for l in reversed(range(L)):
             dx_l = dx_bufs[l & 1]
-            dgrad(dy, 2 * C, bw["w1t"][l], bw["w1t_inv"][l], C, 6 * C,
-                  [(0, dil, 0, 2 * C), (0, 0, 0, 2 * C), (0, -dil, 0, 2 * C)], res_planes=dx_next, res_scale=inv_sqrt2,
-                  out_planes=dx_l, out_f32=dx0 if l == 0 else None)
-            if d_cond is not None:
-                dgrad(dy, 2 * C, bw["wct"][l], bw["wct_inv"][l] * inv_S, E, 2 * C, [(0, 0, 0, 2 * C)], out_f32=d_cond,
-                      out_accum=True)
-            cs_l = colsum(planes=dx_l, Nn=C)
-            dd = cs_l if cs_next is None else cs_l - cs_next * inv_sqrt2               # d wrt the step vector d_l
-            d_d[:, l, :] = dd if Bs > 1 else dd.sum(0, keepdim=True)
-            dx_next, cs_next = dx_l, cs_l
-
-        if direct:
-            gb1_all = cs_dy.sum(1)
-            # conv input is x + d_l (zero padded): sum_t dy[t,r] * d[c] over the steps where tap j reads inside [0,T)
-            if sync is None:
-                _add_step_vector_term(gw1_all, cs_dy, cs_edge, sv["d"].transpose(0, 1), Bs, C)
-            else:
-                sync.wait()            # every bucket reduced before the gradients are laid out for autograd
-            gw2_all[:, :C] *= inv_sqrt2
-            for l in range(L):
-                grads[f"l{l}.w2"] = gw2_all[l]
+            bd.x_planes, bd.y_planes, bd.z_planes = N.ptr(sv["xs"][l]), N.ptr(sv["ys"][l]), N.ptr(sv["zs"][l])
+            bd.dx_next = N.ptr(dx_next)
+            bd.w2t, bd.w1t, bd.wct = N.ptr(bw["w2t"][l]), N.ptr(bw["w1t"][l]), N.ptr(bw["wct"][l])
+            bd.w2t_inv, bd.w1t_inv, bd.wct_inv = bw["w2t_inv"][l], bw["w1t_inv"][l], bw["wct_inv"][l]
+            bd.dx_out, bd.dx_f32 = N.ptr(dx_l), N.ptr(dx0 if l == 0 else None)
+            bd.gw1, bd.gw2 = N.ptr(gw1_all[l]), N.ptr(gw2_all[l])
+            bd.cs_dy, bd.cs_edge, bd.cs_dx = N.ptr(cs_dy[l]), N.ptr(cs_edge[l]), N.ptr(cs_x[l])
+            bd.dilation = pk["dil"][l]
+            N.check(lib.fd_wavenet_block_bwd(ctypes.byref(bd), st), "fd_wavenet_block_bwd")
+            dx_next = dx_l
+            if sync is not None and (l % bucket == 0):
+                # layers [l, hi) are final: add their rank-one step-vector term (it depends on this rank's d) and
+                # start the all-reduce of the bucket; it overlaps the backward of the layers below
+                hi = min(L, l + bucket)
+                _add_step_vector_term(gw1_all[l:hi], cs_dy[l:hi], cs_edge[l:hi], dl_all[l:hi], Bs, C)
+                sync.reduce_async(gw1_all[l:hi], gw2_all[l:hi])
+        d_d = cs_x[:L] - cs_x[1:] * inv_sqrt2                                  # [L,B,C] gradient wrt the step vectors d_l
+        d_d = d_d.transpose(0, 1) if Bs > 1 else d_d.sum(1, keepdim=True).transpose(0, 1)
+        d_d = d_d.contiguous()
+        gb2_all = torch.cat([cs_x[1:].sum(1) * inv_sqrt2, cs_skip.sum(0).expand(L, C)], dim=1)   # [L,2C]
+        gb1_all = cs_dy.sum(1)
+        # conv input is x + d_l (zero padded): sum_t dy[t,r] * d[c] over the steps where tap j reads inside [0,T)
+        if sync is None:
+            _add_step_vector_term(gw1_all, cs_dy, cs_edge, dl_all, Bs, C)
+        else:
+            sync.wait()            # every bucket reduced before the gradients are laid out for autograd
+        gw2_all[:, :C] *= inv_sqrt2
+        for l in range(L):
+            grads[f"l{l}.w2"], grads[f"l{l}.b2"] = gw2_all[l], gb2_all[l]
 
         # packed -> reference layouts for all layers at once
         gw1_o = torch.empty_like(gw1_all)
@@ -345,10 +259,7 @@ class WaveNetTrainFn(torch.autograd.Function):
         # dx_next now is d(x_0) where x_0 = relu(input_projection(x)): mask with x_0 > 0
         dx0m = torch.empty((2, B, T, C), **i16)
         N.check(lib.fd_relu_bwd(N.ptr(dx0), N.ptr(sv["xs"][0]), N.ptr(dx0m), rows * C, 1.0, prec, st), "fd_relu_bwd")
-        if direct:
-            grads["input_projection.w"] = wgrad_direct([dx0m], [(0, 0, C)], [sv["x_planes"]], [(0, 0, 0, M)])
-        else:
-            grads["input_projection.w"] = wgrad(fold(dx0m, C), C, fold(sv["x_planes"], M), M)
+        grads["input_projection.w"] = wgrad(dx0m, C, sv["x_planes"], M)
         grads["input_projection.b"] = colsum(planes=dx0m, Nn=C).sum(0)
         d_x = None
         if ctx.need_x:     # d(x) = d(x_0 masked by the ReLU) . W_in   (wavenet.py:211)

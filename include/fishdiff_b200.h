@@ -32,7 +32,7 @@ extern "C" {
 #define FD_PREC_SINGLE 0x10
 #define FD_BACKEND_TC 0
 #define FD_BACKEND_SIMT 1
-#define FD_ABI_VERSION 1
+#define FD_ABI_VERSION 2
 
 /* ------------------------------------------------------------------------------------------- misc */
 int fd_abi_version(void);
@@ -261,20 +261,15 @@ int fd_stft_mag_eps_fwd(const uint16_t* padded, const uint16_t* dft_w, uint16_t*
 int fd_log_clamp(const float* x, float* y, long long n, float clip, float out_scale, void* stream);
 
 /* ------------------------------------------------------------------ training step (a8): backward of the denoiser */
-/* General linear tap-GEMM: up to two source tensors, explicit source strides (0 = canonical [2][B][T][C]), a K offset
- * on the W operand (w_kshift + b*w_bstride_k).  It expresses every gradient GEMM of the WaveNet backward:
- *   data gradients: transposed packed weights, mirrored tap shifts, two sources ([dx_next | d_skip]);
- *   weight gradients: src = folded transpose of the output gradient ("rows" = output channels, C = padded time),
- *                     W = folded transpose of the forward input, w_kshift = tap shift, w_bstride_k = Tp,
- *                     out_f32 [B][rows][cols] holds one partial per batch item (reduced by fd_reduce_batch).
+/* General linear tap-GEMM: up to two source tensors [2][B][T][src_C], and a K offset w_kshift on the W operand (a
+ * multiple of 8; selects a column block of W, e.g. the skip half of W2^T).  The data gradients of the WaveNet backward
+ * use it with transposed packed weights, mirrored tap shifts and two sources ([dx_next | d_skip]).
  * Epilogue = the LINEAR epilogue of fd_conv_cl_fwd plus res_scale on the res_planes term. */
 typedef struct fd_gemm_desc {
   const uint16_t* src[2];
   int src_C[2];
-  long long src_rs[2], src_bs[2], src_ps[2];
   const uint16_t* w;
   int n_total, k_total, w_kshift;
-  long long w_bstride_k;
   int B, T, num_seg;
   int seg_src[16], seg_shift[16], seg_coff[16], seg_klen[16];
   const float* bias;
@@ -313,14 +308,6 @@ int fd_wavenet_block_fwd_train(const uint16_t* x_planes, uint16_t* x_out_planes,
  * diffusion projections run under torch autograd on [Bs,C]-sized tensors) */
 int fd_wavenet_gate_bias_from_d(const float* d, const float* w1p, const float* bias_sum, float* gb_full, float* gb_lo,
                                 float* gb_hi, int L, int Bs, int C, int KT, void* stream);
-/* planes [2][B][T][C] -> planes [2][C][B][Tp] (item b at columns [pad, pad+T) of its Tp span, zeros elsewhere).
- * mode 0: value*scale (+ addvec[b*add_bstride + c]); mode 1: src is a packed pre-activation tensor with 2C columns,
- * value = sigmoid(g)*tanh(f); mode 2: value = src_f32 * (aux_planes > 0) (ReLU backward).
- * The C rows may be written at row offset dst_row0 of a taller destination with dst_rows rows (stacked operands of the
- * weight-gradient GEMMs); dst_rows <= 0 means dst_rows = C, dst_row0 = 0. */
-int fd_fold_transpose(const uint16_t* src_planes, const float* src_f32, const uint16_t* aux_planes, const float* addvec,
-                      int add_bstride, uint16_t* dst, int B, int T, int C, int Tp, int pad, float scale, int mode,
-                      int gate_tile, int prec, int dst_rows, int dst_row0, void* stream);
 /* backward of z = sigmoid(g)*tanh(f) (wavenet.py:114-115): dz fp32 [rows][C], y planes [2][rows][2C] -> dy planes */
 int fd_gate_bwd(const float* dz, const uint16_t* y_planes, uint16_t* dy_planes, long long rows, int C, int gate_tile,
                 int prec, void* stream);
@@ -344,12 +331,14 @@ int fd_colsum(const uint16_t* planes, const float* f32, float* out, int B, int T
 int fd_colsum_edges(const uint16_t* planes, float* out, int B, int T, int N, int e, float scale, int prec,
                     void* stream);
 
-/* Weight gradient straight from channels-last split planes, no transposes (wgmma with MN-major operands):
+/* Weight gradient straight from channels-last split planes, no transposes:
  *   part[s][r][c] = acc_scale * sum_{b in split s} sum_t ROW[b,t,r] * COL[b,t+shift(c),c]
  * Rows r are the concatenation of 1..2 row segments, columns c of 1..8 column segments; a segment names a source
- * tensor (planes [2][B][T][C_src]), its first channel, its width (multiple of 64) and -- columns only -- a time shift
+ * tensor (planes [2][B][T][C_src]), its first channel (a multiple of 8), its width and -- columns only -- a time shift
  * (rows outside [0,T) read as zero: the conv zero padding of that tap).  Items are divided over `splits` partials
  * (1 <= splits <= B; ceil(B/splits) consecutive items each) which the caller sums with fd_reduce_batch.
+ * backend FD_BACKEND_TC: wgmma with MN-major operands, segment widths multiples of 64; FD_BACKEND_SIMT: fp32 FFMA twin,
+ * segment widths multiples of 8.
  * Replaces autograd's conv-weight gradient of modules/wavenet.py:106-120 (reference runs it through cuDNN wgrad).
  * `prec` may carry FD_PREC_SINGLE. */
 typedef struct fd_wgrad_desc {
@@ -365,6 +354,7 @@ typedef struct fd_wgrad_desc {
   float* part;        /* [splits][R][Cc] fp32, R / Cc = total row / column widths */
   float acc_scale;
   int prec;
+  int backend;
 } fd_wgrad_desc;
 int fd_wgrad_cl(const fd_wgrad_desc* d, void* stream);
 
@@ -374,7 +364,8 @@ int fd_reduce_batch(const float* in, float* out, int B, long long n, float scale
 /* Backward of ONE ResidualBlock (autograd of modules/wavenet.py:106-120) as one native call: the 5 GEMM launches and the
  * elementwise / reduction kernels around them, issued back to back on `stream`:
  *   dz   = [dx_next/sqrt2 | d_skip] . W2            (fd_gemm_cl_fwd, two sources; skip half only above the last layer)
- *   dy   = gate backward of dz on the saved pre-activations (fd_gate_bwd)
+ *   dy   = gate backward of dz on the saved pre-activations (fused into the dz GEMM's epilogue on FD_BACKEND_TC;
+ *          fd_gate_bwd, fd_colsum and fd_colsum_edges after a plain dz GEMM into the `dz` workspace on FD_BACKEND_SIMT)
  *   gw2  = [dx_next ; d_skip]^T . z                  (fd_wgrad_cl + fd_reduce_batch; the 1/sqrt2 of the residual rows is
  *                                                     applied by the caller to all layers at once)
  *   gw1  = dy^T . [x(t-d) | x(t) | x(t+d) | cond]   (one weight-gradient GEMM, packed row order)
@@ -382,7 +373,8 @@ int fd_reduce_batch(const float* in, float* out, int B, long long n, float scale
  *   dx   = conv^T(dy) + dx_next/sqrt2 -> planes (+ fp32 copy when dx_f32 != NULL);  d_cond += dy . Wc;  cs_dx = colsum(dx)
  * All gradients inside the chain carry the caller's power-of-two scale S; results that leave it are multiplied by
  * inv_S.  cs_dy [B][2C], cs_edge [2][B][2C], cs_dx [B][C] must be zero on entry.  part1 / part2: fp32 workspaces of
- * splits1*2C*(3C+E) and splits2*2C*C floats.  Needs C, E multiples of 64 (the direct weight-gradient kernel). */
+ * splits1*2C*(3C+E) and splits2*2C*C floats.  C and E must be multiples of 64 on FD_BACKEND_TC (the wgmma
+ * weight-gradient kernel), multiples of 8 on FD_BACKEND_SIMT. */
 typedef struct fd_wavenet_bwd_desc {
   const uint16_t* x_planes;    /* xs[l]   [2][B][T][C]  residual stream entering the layer */
   const uint16_t* y_planes;    /* ys[l]   [2][B][T][2C] gate/filter pre-activations, packed order */
