@@ -152,12 +152,13 @@ class PitchAdjustableMelSpectrogram:
             padded = torch.zeros((2, B, pitch), dtype=torch.int16, device=dev)
             if pitch == (Np + 7) // 8 * 8:
                 N.check(lib.fd_reflect_pad_split(N.ptr(y), N.ptr(padded), B, n, pad, prec, st), "fd_reflect_pad_split")
-                np_arg = Np
             else:
                 tmp = torch.zeros((2, B, (Np + 7) // 8 * 8), dtype=torch.int16, device=dev)
                 N.check(lib.fd_reflect_pad_split(N.ptr(y), N.ptr(tmp), B, n, pad, prec, st), "fd_reflect_pad_split")
                 padded[:, :, :tmp.shape[2]] = tmp
-                np_arg = pitch
+            # the rows span the whole pitch (zeros past Np): under key shift the last frame's K padding can end inside
+            # the 8-element tail of the padded signal (kpad - n_fft_new = 2 at -5, 18 at +5)
+            np_arg = pitch
             row_stride = hop
         else:
             # arbitrary hop (time-stretch augmentation draws e.g. 512*1.1 = 563): the frames are gathered once into an
