@@ -30,9 +30,6 @@
 
 namespace {
 
-constexpr int RP_CONSUMER_THREADS = 256;
-constexpr int RP_THREADS = RP_CONSUMER_THREADS + 128;     // + the producer warpgroup
-
 struct FdResPairK {
   int B, T;
   int k1, d1, k2;
@@ -74,17 +71,13 @@ struct RpCfg {
   static constexpr int MID_PLANE_BYTES = MID_ROWS * ROWB;
   static constexpr int MID_KB_BYTES = 2 * MID_PLANE_BYTES;
   static constexpr int MID_BYTES = NKB * MID_KB_BYTES;     // c1 output; afterwards the staging image of the output
-  static constexpr int MAX_STAGES = 8;
   static constexpr int HEAD_BYTES = 2048;                   // biases (2C floats <= 1 KB) + barriers, in front of the tiles
-  static constexpr int SMEM_BYTES = 227 * 1024;             // the ring takes what the tiles leave
-  static constexpr int FIXED_MAX = 1024 + HEAD_BYTES + NKB * 2 * RIN_MAX * ROWB + MID_BYTES;
-  static_assert((SMEM_BYTES - FIXED_MAX) / (GROUP * UNIT_BYTES) >= 2, "weight ring needs two stages");
-  static_assert(2 * C * 4 + (2 * MAX_STAGES + 2) * 8 <= HEAD_BYTES, "head region too small");
-  // stages of the weight ring for an input tile of r_in rows
+  static_assert(2 * C * 4 + (2 * FD_TC_MAX_STAGES + 2) * 8 <= HEAD_BYTES, "head region too small");
+  // stages of the weight ring for an input tile of r_in rows: the ring takes what the tiles leave of FD_TC_SMEM_BUDGET
   static constexpr int stages_for(int r_in, int group) {
-    const int n = (SMEM_BYTES - 1024 - HEAD_BYTES - NKB * 2 * r_in * ROWB - MID_BYTES) / (group * UNIT_BYTES);
-    return n > MAX_STAGES ? MAX_STAGES : n;
+    return fd_tc_ring_stages(1024 + HEAD_BYTES + NKB * 2 * r_in * ROWB + MID_BYTES, group * UNIT_BYTES);
   }
+  static_assert(stages_for(RIN_MAX, GROUP) >= 2, "weight ring needs two stages");
 };
 
 __device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t mask) { return off ^ (((off >> 7) & mask) << 4); }
@@ -109,7 +102,7 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sm
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"r"(RP_CONSUMER_THREADS) : "memory"); }
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory"); }
 
 // One conv of the pair over the whole tile: acc[j] (block j of this warpgroup) += A(shifted rows) x W for every listed
 // weight unit.  A comes from the swizzled activation tile at a_base (a_kb bytes per 64-channel block, a_plane bytes
@@ -176,7 +169,7 @@ __device__ __forceinline__ void rp_gemm(float* acc, const FdResPairK& p, int uni
 }
 
 template <int C, int PREC>
-__global__ void __launch_bounds__(RP_THREADS, 1)
+__global__ void __launch_bounds__(FD_TC_THREADS, 1)
 fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w1,
                      const __grid_constant__ CUtensorMap tm_w2, const __grid_constant__ CUtensorMap tm_out,
                      const __grid_constant__ CUtensorMap tm_out_last, const FdResPairK p) {
@@ -186,8 +179,8 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* bias_s = reinterpret_cast<float*>(smem);                  // b1 [C] | b2 * s2 [C]
   uint64_t* w_full = reinterpret_cast<uint64_t*>(bias_s + 2 * C);
-  uint64_t* w_empty = w_full + K::MAX_STAGES;
-  uint64_t* in_full = w_empty + K::MAX_STAGES;
+  uint64_t* w_empty = w_full + FD_TC_MAX_STAGES;
+  uint64_t* in_full = w_empty + FD_TC_MAX_STAGES;
   uint64_t* in_empty = in_full + 1;
   const int in_plane = p.r_in * K::ROWB;                           // multiple of the swizzle period (rows % 8 == 0)
   const int in_kb = 2 * in_plane;
@@ -202,11 +195,11 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
   const int num_tiles = p.B * tiles_t;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.nstages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], RP_CONSUMER_THREADS / 32); }
-    mbar_init(in_full, 1); mbar_init(in_empty, RP_CONSUMER_THREADS / 32);
+    for (int i = 0; i < p.nstages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], FD_TC_CONSUMER_THREADS / 32); }
+    mbar_init(in_full, 1); mbar_init(in_empty, FD_TC_CONSUMER_THREADS / 32);
     fence_barrier_init();
   }
-  if (warp == 8 && lane == 0) {
+  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
     prefetch_tmap(&tm_in); prefetch_tmap(&tm_w1); prefetch_tmap(&tm_w2); prefetch_tmap(&tm_out); prefetch_tmap(&tm_out_last);
   }
   // biases (b2 pre-multiplied by the weight prescale of c2); the 16 trailing rows of the mid tile are zero for the whole kernel
@@ -216,8 +209,8 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
         make_uint4(0, 0, 0, 0);
   __syncthreads();
 
-  if (warp >= 8) producer_regs();
-  if (warp == 8) {
+  if (warp >= FD_TC_PRODUCER_WARP) producer_regs();
+  if (warp == FD_TC_PRODUCER_WARP) {
     // =========================================================== weight producer (the pair's weights, once per tile)
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
@@ -244,9 +237,9 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
     }
     return;
   }
-  if (warp >= 9) {
+  if (warp >= FD_TC_PRODUCER_WARP + 1) {
     // =========================================================== activation-tile producer
-    if (warp == 9 && lane == 0) {
+    if (warp == FD_TC_PRODUCER_WARP + 1 && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
         const int b = tile / tiles_t, t0 = (tile % tiles_t) * p.r_out;
@@ -383,42 +376,6 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
 }
 
 // ------------------------------------------------------------------ host side
-CUtensorMapSwizzle swizzle_for_bytes(int row_bytes) {
-  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                                                         : CU_TENSOR_MAP_SWIZZLE_32B;
-}
-
-// planes [2][B][T][C] (uint16): box {bk, rows, 1, nplanes}
-int make_planes_map(CUtensorMap* m, const uint16_t* ptr, int B, int T, int C, int bk, int rows, int nplanes) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)B, 2};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)T * C * 2, (cuuint64_t)B * T * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)rows, 1, (cuuint32_t)nplanes};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<uint16_t*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_bytes(bk * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(planes) failed: %d (B=%d T=%d C=%d bk=%d rows=%d)", (int)r, B, T,
-             C, bk, rows);
-  return 0;
-}
-
-// packed weights [2][C][K] (uint16): box {bkw, C, planes} (both planes of a unit, or one per CTA of a multicast pair)
-int make_wpair_map(CUtensorMap* m, const uint16_t* ptr, int C, int Ktot, int bkw, int planes) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)Ktot, (cuuint64_t)C, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)Ktot * 2, (cuuint64_t)C * Ktot * 2};
-  cuuint32_t box[3] = {(cuuint32_t)bkw, (cuuint32_t)C, (cuuint32_t)planes};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<uint16_t*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_bytes(bkw * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(w pair) failed: %d (C=%d K=%d)", (int)r, C, Ktot);
-  return 0;
-}
-
 template <int C, int PREC>
 int launch_respair(const fd_respair_desc& d, FdResPairK p, cudaStream_t stream) {
   using K = RpCfg<C>;
@@ -433,34 +390,22 @@ int launch_respair(const fd_respair_desc& d, FdResPairK p, cudaStream_t stream) 
   // mean fewer barrier round trips per tile
   p.group = K::stages_for(p.r_in, 2 * K::GROUP) >= 2 ? 2 * K::GROUP : K::GROUP;
   p.nstages = K::stages_for(p.r_in, p.group);
+  // planes [2][B][T][C], one plane per box; weights [2][C][k C], both planes of a unit in one box
+  const long long rs = C, is = (long long)p.T * C, ps = (long long)p.B * p.T * C;
   CUtensorMap tin, tw1, tw2, tout, tout_last;
-  int rc = make_planes_map(&tin, d.in_planes, p.B, p.T, C, K::BK_A, p.rb, 1);
+  int rc = planes_map(&tin, d.in_planes, C, p.T, p.B, rs, is, ps, K::BK_A, p.rb, 1, "respair in");
   if (rc) return rc;
-  rc = make_wpair_map(&tw1, d.w1, C, p.k1 * C, K::BKW, 2);
+  rc = weights_map(&tw1, d.w1, C, p.k1 * C, K::BKW, C, 2, "respair w1");
   if (rc) return rc;
-  rc = make_wpair_map(&tw2, d.w2, C, p.k2 * C, K::BKW, 2);
+  rc = weights_map(&tw2, d.w2, C, p.k2 * C, K::BKW, C, 2, "respair w2");
   if (rc) return rc;
-  rc = make_planes_map(&tout, d.out_planes, p.B, p.T, C, K::BK_A, 128, 1);
+  rc = planes_map(&tout, d.out_planes, C, p.T, p.B, rs, is, ps, K::BK_A, 128, 1, "respair out");
   if (rc) return rc;
-  rc = make_planes_map(&tout_last, d.out_planes, p.B, p.T, C, K::BK_A, 128 - (p.k2 - 1), 1);
+  rc = planes_map(&tout_last, d.out_planes, C, p.T, p.B, rs, is, ps, K::BK_A, 128 - (p.k2 - 1), 1, "respair out_last");
   if (rc) return rc;
-  auto kern = fd_respair_tc_kernel<C, PREC>;
-  static bool attr_set[FD_MAX_DEVICES] = {false};
-  const int dev = fd_current_device();
-  if (!attr_set[dev]) {
-    FD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM_BYTES));
-    FD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    attr_set[dev] = true;
-  }
   const int tiles = p.B * ((p.T + p.r_out - 1) / p.r_out);
-  const int sms = fd_device_sms(dev);
-  const int grid = tiles < sms ? tiles : sms;
-  fd_prof_begin(C == 128 ? 12 : C == 64 ? 13 : C == 32 ? 14 : 15, stream);
-  kern<<<grid, RP_THREADS, K::SMEM_BYTES, stream>>>(tin, tw1, tw2, tout, tout_last, p);
-  fd_prof_end(stream);
-  FD_CHECK_CUDA(cudaGetLastError());
-  fd_count_launch(1);
-  return 0;
+  return fd_tc_launch<fd_respair_tc_kernel<C, PREC>>(FD_TC_SMEM_BUDGET, tiles, stream, true, tin, tw1, tw2, tout,
+                                                     tout_last, p);
 }
 
 template <int C>
@@ -522,10 +467,15 @@ extern "C" int fd_respair_fwd(const fd_respair_desc* d, void* stream) {
     p.masked1 = m1 ? 1 : 0; p.masked2 = m2 ? 1 : 0;
   }
   cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  fd_prof_begin(d->C == 128 ? 12 : d->C == 64 ? 13 : d->C == 32 ? 14 : 15, st);
   switch (d->C) {
-    case 128: return launch_respair_prec<128>(*d, p, st);
-    case 64: return launch_respair_prec<64>(*d, p, st);
-    case 32: return launch_respair_prec<32>(*d, p, st);
-    default: return launch_respair_prec<16>(*d, p, st);
+    case 128: rc = launch_respair_prec<128>(*d, p, st); break;
+    case 64: rc = launch_respair_prec<64>(*d, p, st); break;
+    case 32: rc = launch_respair_prec<32>(*d, p, st); break;
+    default: rc = launch_respair_prec<16>(*d, p, st); break;
   }
+  fd_prof_end(st);
+  if (rc == 0) fd_count_launch(1);
+  return rc;
 }

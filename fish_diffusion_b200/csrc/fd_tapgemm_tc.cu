@@ -22,15 +22,11 @@
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int CONSUMER_THREADS = 256;                 // two warpgroups
-constexpr int PRODUCER_WARP = CONSUMER_THREADS / 32;
-constexpr int NUM_THREADS = CONSUMER_THREADS + 128;     // + the producer warpgroup
-constexpr int SCRATCH_BYTES = (CONSUMER_THREADS / 32) * 2048;   // the consumer warps' epilogue scratch
 
 // ring stages of `stage_bytes` that fit next to the fixed parts of shared memory (bias vectors, barriers, scratch)
 constexpr int ring_stages(int stage_bytes, int bias_floats) {
-  const int n = (227 * 1024 - (1024 /*align slack*/ + bias_floats * 4 + 2 * 8 * 8 + SCRATCH_BYTES)) / stage_bytes;
-  return n > 8 ? 8 : n;
+  return fd_tc_ring_stages(1024 /*align slack*/ + bias_floats * 4 + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES,
+                           stage_bytes);
 }
 
 // NPL = operand planes staged per k-block: 2 (hi + lo, three products) or 1 (hi only, one product: 11-bit (f16) /
@@ -55,13 +51,13 @@ struct Cfg {
   static constexpr int BIAS_FLOATS = (EPI == FD_EPI_GATE ? 3 : 1) * BLOCK_N;
   static constexpr int NUM_STAGES = ring_stages(STAGE_BYTES, BIAS_FLOATS);
   static constexpr int SMEM_BYTES = 1024 /*align slack*/ + NUM_STAGES * STAGE_BYTES + BIAS_FLOATS * 4 +
-                                    2 * NUM_STAGES * 8 + SCRATCH_BYTES;
+                                    2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
   static_assert(NUM_STAGES >= 2, "pipeline needs at least two stages");
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
+  static_assert(SMEM_BYTES <= FD_TC_SMEM_BUDGET, "shared memory");
 };
 
 template <int BLOCK_N, int BLOCK_K, int EPI, int PREC, int NPL>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(FD_TC_THREADS, 1)
 fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_constant__ CUtensorMap tm_src1,
                      const __grid_constant__ CUtensorMap tm_w, const FdTapGemm p) {
   using C = Cfg<BLOCK_N, BLOCK_K, EPI, NPL>;
@@ -85,20 +81,20 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   for (int sI = 0; sI < p.num_seg; ++sI) total_k_blocks += p.seg[sI].k_len / BLOCK_K;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_THREADS / 32); }
+    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], FD_TC_CONSUMER_THREADS / 32); }
     fence_barrier_init();
   }
-  if (warp == PRODUCER_WARP && lane == 0) {
+  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
     prefetch_tmap(&tm_src0);
     prefetch_tmap(&tm_src1);
     prefetch_tmap(&tm_w);
   }
   __syncthreads();
 
-  if (warp >= PRODUCER_WARP) {
+  if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
     producer_regs();
-    if (warp == PRODUCER_WARP && lane == 0) {
+    if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_tile = tile / num_n_tiles;
@@ -134,7 +130,7 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   consumer_regs();
   const int wg = warp / 4;                                   // rows [64 wg, 64 wg + 64) of the tile
   const int wq = warp % 4;                                   // 16-row slice of the warpgroup's 64 rows
-  const uint32_t my_scratch = smem_u32(scratch_s) + warp * 2048;
+  const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
   float acc[BLOCK_N / 2];
   int stage = 0; uint32_t phase = 0;
   long long staged_key = -1;                                 // which bias vectors shared memory holds
@@ -151,19 +147,19 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
                                                   : (long long)b * p.bias_bstride + n0;
     if (EPI != FD_EPI_MAG && EPI != FD_EPI_GATE_BWD && bias_key != staged_key) {
       staged_key = bias_key;
-      asm volatile("bar.sync 1, %0;" ::"r"(CONSUMER_THREADS) : "memory");
+      asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory");
       if (EPI == FD_EPI_GATE) {
         const size_t bo = (size_t)b * p.gbias_bstride + n0;
-        for (int i = threadIdx.x; i < BLOCK_N; i += CONSUMER_THREADS) {
+        for (int i = threadIdx.x; i < BLOCK_N; i += FD_TC_CONSUMER_THREADS) {
           bias_s[i] = p.gbias_full[bo + i];
           bias_s[BLOCK_N + i] = p.gbias_lo[bo + i];
           bias_s[2 * BLOCK_N + i] = p.gbias_hi[bo + i];
         }
       } else {
-        for (int i = threadIdx.x; i < BLOCK_N; i += CONSUMER_THREADS)
+        for (int i = threadIdx.x; i < BLOCK_N; i += FD_TC_CONSUMER_THREADS)
           bias_s[i] = p.bias ? p.bias[(size_t)b * p.bias_bstride + n0 + i] : 0.f;
       }
-      asm volatile("bar.sync 1, %0;" ::"r"(CONSUMER_THREADS) : "memory");
+      asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory");
     }
 
     // ---- mainloop: one wgmma group per ring stage, one group kept in flight; a stage is released once the group
@@ -555,72 +551,24 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
 }
 
 // ------------------------------------------------------------------ host side
-CUtensorMapSwizzle swizzle_for(int block_k) {
-  return block_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : block_k == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                                                      : CU_TENSOR_MAP_SWIZZLE_32B;
-}
-
-int make_src_map(CUtensorMap* m, const uint16_t* ptr, int B, int T, int C, long long rs, long long bs,
-                 long long ps, int block_k, int npl) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)B, 2};
-  cuuint64_t strides[3] = {(cuuint64_t)rs * 2, (cuuint64_t)bs * 2, (cuuint64_t)ps * 2};
-  cuuint32_t box[4] = {(cuuint32_t)block_k, (cuuint32_t)BLOCK_M, 1, (cuuint32_t)npl};   // planes in one box
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<uint16_t*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(block_k), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(src) failed: %d (B=%d T=%d C=%d bk=%d ptr=%p)", (int)r, B,
-             T, C, block_k, (const void*)ptr);
-  return 0;
-}
-
-int make_w_map(CUtensorMap* m, const uint16_t* ptr, int N, int K, int block_n, int block_k, int npl) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)N, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)N * K * 2};
-  cuuint32_t box[3] = {(cuuint32_t)block_k, (cuuint32_t)block_n, (cuuint32_t)npl};   // planes in one box
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<uint16_t*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(block_k), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(w) failed: %d (N=%d K=%d bn=%d bk=%d)", (int)r, N, K,
-             block_n, block_k);
-  return 0;
-}
-
-
 template <int BLOCK_N, int BLOCK_K, int EPI, int PREC, int NPL>
 int launch_inst(const FdTapGemm& p, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N, BLOCK_K, EPI, NPL>;
-  CUtensorMap tm0, tm1, tmw;
-  int rc = make_src_map(&tm0, p.src[0], p.B, p.T, p.src_C[0], p.src_rs[0], p.src_bs[0], p.src_ps[0], BLOCK_K, NPL);
+  CUtensorMap tm0, tm1, tmw;   // the hi and lo planes of an operand arrive in one box
+  int rc = planes_map(&tm0, p.src[0], p.src_C[0], p.T, p.B, p.src_rs[0], p.src_bs[0], p.src_ps[0], BLOCK_K, BLOCK_M,
+                      NPL, "tapgemm src0");
   if (rc) return rc;
   if (p.src[1] != nullptr) {
-    rc = make_src_map(&tm1, p.src[1], p.B, p.T, p.src_C[1], p.src_rs[1], p.src_bs[1], p.src_ps[1], BLOCK_K, NPL);
+    rc = planes_map(&tm1, p.src[1], p.src_C[1], p.T, p.B, p.src_rs[1], p.src_bs[1], p.src_ps[1], BLOCK_K, BLOCK_M, NPL,
+                    "tapgemm src1");
     if (rc) return rc;
   } else {
     tm1 = tm0;
   }
-  rc = make_w_map(&tmw, p.w, p.n_total, p.k_total, BLOCK_N, BLOCK_K, NPL);
+  rc = weights_map(&tmw, p.w, p.n_total, p.k_total, BLOCK_K, BLOCK_N, NPL, "tapgemm w");
   if (rc) return rc;
-
-  auto kern = fd_tapgemm_tc_kernel<BLOCK_N, BLOCK_K, EPI, PREC, NPL>;
-  static bool attr_set[FD_MAX_DEVICES] = {false};   // the max-dynamic-smem attribute is per device
-  const int dev = fd_current_device();
-  if (!attr_set[dev]) {
-    FD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set[dev] = true;
-  }
-  const int g_num_sms = fd_device_sms(dev);
-  const int tiles_t = (p.T + BLOCK_M - 1) / BLOCK_M;
-  const int num_tiles = p.B * tiles_t * (p.n_total / BLOCK_N);
-  const int grid = num_tiles < g_num_sms ? num_tiles : g_num_sms;
-  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tm0, tm1, tmw, p);
-  FD_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  const int num_tiles = p.B * ((p.T + BLOCK_M - 1) / BLOCK_M) * (p.n_total / BLOCK_N);
+  return fd_tc_launch<fd_tapgemm_tc_kernel<BLOCK_N, BLOCK_K, EPI, PREC, NPL>>(
+      Cfg<BLOCK_N, BLOCK_K, EPI, NPL>::SMEM_BYTES, num_tiles, stream, false, tm0, tm1, tmw, p);
 }
 
 template <int BLOCK_N, int BLOCK_K, int EPI>

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "fd_common.cuh"
+#include "fd_host.h"
 
 namespace {
 
@@ -76,8 +77,21 @@ __device__ __forceinline__ void sts64(uint32_t addr, float x, float y) {
 // Register budget of a warp-specialised CTA of three warpgroups (384 threads: at most 168 registers per thread at launch):
 // the producer warpgroup, which only issues TMA, hands its registers to the two consumer warpgroups, which hold the
 // accumulators (128 x 40 + 256 x 232 = 64512 of the 65536 registers of an SM).  Every thread of a warpgroup executes it.
+// Warps 0..7 are the consumers, warps 8..11 the producer warpgroup.
+constexpr int FD_TC_CONSUMER_THREADS = 256;
+constexpr int FD_TC_THREADS = FD_TC_CONSUMER_THREADS + 128;
+constexpr int FD_TC_PRODUCER_WARP = FD_TC_CONSUMER_THREADS / 32;
 __device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory"); }
 __device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory"); }
+
+// Dynamic shared memory of one CTA per SM (227 KB on sm_90), and the pipeline ring that fills what the fixed parts of a
+// kernel's layout leave: stages of `stage_bytes` in FD_TC_SMEM_BUDGET - `fixed_bytes`, at most FD_TC_MAX_STAGES.
+constexpr int FD_TC_SMEM_BUDGET = 227 * 1024;
+constexpr int FD_TC_MAX_STAGES = 8;
+constexpr int fd_tc_ring_stages(int fixed_bytes, int stage_bytes) {
+  const int n = (FD_TC_SMEM_BUDGET - fixed_bytes) / stage_bytes;
+  return n > FD_TC_MAX_STAGES ? FD_TC_MAX_STAGES : n;
+}
 
 // ------------------------------------------------------------------ wgmma
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -108,6 +122,11 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
 // swizzle mode of a K-major operand whose rows are `row_bytes` long (128 / 64 / 32)
 __host__ __device__ constexpr uint32_t swizzle_mode_for(int row_bytes) {
   return row_bytes == 128 ? 1u : row_bytes == 64 ? 2u : 3u;
+}
+// the TMA swizzle that writes what that descriptor reads; NONE for other row lengths, which encode_tiled refuses
+CUtensorMapSwizzle tma_swizzle_for(int row_bytes) {
+  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+         : row_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
 }
 
 // wgmma.mma_async m64nNk16, fp32 accumulators d[N/2] in the standard fragment layout (see frag_to_scratch).
@@ -480,6 +499,8 @@ template <> struct Wgmma<256, FD_BF16> {
 //   row = l/4 + 8 ((i/2) % 2),  col = 8 (i/4) + 2 (l % 4) + (i % 2).
 // The epilogues re-distribute a chunk of columns through a warp-private 16 x 32 fp32 scratch (2 KB; 16-byte chunks
 // XOR-swizzled by row & 7) into whatever per-lane layout their global accesses want.
+constexpr int FD_TC_SCRATCH_WARP_BYTES = 16 * 32 * 4;
+constexpr int FD_TC_SCRATCH_BYTES = (FD_TC_CONSUMER_THREADS / 32) * FD_TC_SCRATCH_WARP_BYTES;   // all consumer warps
 // Writes columns [c0, c0 + CW) of the fragment (d points at the tile's first register) to scratch columns
 // [off, off + CW).
 template <int CW>
@@ -512,6 +533,65 @@ PFN_tmapEncodeTiled get_encode() {
       fn = reinterpret_cast<PFN_tmapEncodeTiled>(ptr);
   }
   return fn;
+}
+
+// A tensor map over 16-bit split planes (dims, byte strides and box innermost first); the swizzle follows the box's row
+// length, so that it matches swizzle_mode_for of the operand the box lands in.
+int encode_tiled(CUtensorMap* m, const uint16_t* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                 const cuuint32_t* box, const char* what) {
+  PFN_tmapEncodeTiled enc = get_encode();
+  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
+  const CUtensorMapSwizzle sw = tma_swizzle_for((int)box[0] * 2);
+  FD_REQUIRE(sw != CU_TENSOR_MAP_SWIZZLE_NONE, "tensor map (%s): box rows of %u bytes (wgmma swizzles 128, 64 or 32)",
+             what, box[0] * 2);
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, (cuuint32_t)rank, const_cast<uint16_t*>(ptr), dims, strides, box,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(%s) failed: %d (dims %llu x %llu x %llu x %llu, box %u x %u x %u x %u, ptr %p)",
+             what, (int)r, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+             rank == 4 ? (unsigned long long)dims[3] : 1ull, box[0], box[1], box[2], rank == 4 ? box[3] : 1u,
+             (const void*)ptr);
+  return 0;
+}
+
+// Split planes [plane][B][T][C] (strides in elements) as the 4-D tensor (C, T, B, plane); box {box_c, box_rows, 1,
+// box_planes}.
+int planes_map(CUtensorMap* m, const uint16_t* ptr, int C, int T, int B, long long row_stride, long long item_stride,
+               long long plane_stride, int box_c, int box_rows, int box_planes, const char* what) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)B, 2};
+  const cuuint64_t strides[3] = {(cuuint64_t)row_stride * 2, (cuuint64_t)item_stride * 2, (cuuint64_t)plane_stride * 2};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_rows, 1, (cuuint32_t)box_planes};
+  return encode_tiled(m, ptr, 4, dims, strides, box, what);
+}
+
+// Packed weights [plane][N][K] as the 3-D tensor (K, N, plane); box {box_k, box_n, box_planes}.
+int weights_map(CUtensorMap* m, const uint16_t* ptr, int N, int K, int box_k, int box_n, int box_planes,
+                const char* what) {
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)N, 2};
+  const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)N * K * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)box_n, (cuuint32_t)box_planes};
+  return encode_tiled(m, ptr, 3, dims, strides, box, what);
+}
+
+// Launches a persistent kernel of FD_TC_THREADS threads: one CTA per SM, at most one per work unit.  The dynamic
+// shared-memory limit is an attribute of each kernel and device, set on the kernel's first launch on a device (the
+// cache below is per Kern); `max_carveout` also asks for the largest shared-memory carveout.
+template <auto Kern, typename... Args>
+int fd_tc_launch(int smem_bytes, int work_units, cudaStream_t stream, bool max_carveout, const Args&... args) {
+  static bool attr_set[FD_MAX_DEVICES] = {false};
+  const int dev = fd_current_device();
+  if (!attr_set[dev]) {
+    FD_CHECK_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    if (max_carveout)
+      FD_CHECK_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                         cudaSharedmemCarveoutMaxShared));
+    attr_set[dev] = true;
+  }
+  const int sms = fd_device_sms(dev);
+  Kern<<<work_units < sms ? work_units : sms, FD_TC_THREADS, smem_bytes, stream>>>(args...);
+  FD_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 

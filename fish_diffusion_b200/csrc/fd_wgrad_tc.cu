@@ -23,9 +23,6 @@ namespace {
 
 constexpr int WG_BLOCK_M = 128;
 constexpr int WG_BLOCK_K = 64;                 // time steps per pipeline stage
-constexpr int WG_CONSUMER_THREADS = 256;
-constexpr int WG_PRODUCER_WARP = WG_CONSUMER_THREADS / 32;
-constexpr int WG_THREADS = WG_CONSUMER_THREADS + 128;     // + the producer warpgroup
 constexpr int WG_BOX_BYTES = 64 * 64 * 2;      // one plane of one [64 t][64 ch] box
 
 template <int BLOCK_N, int NPL>
@@ -35,15 +32,15 @@ struct WgCfg {
   static constexpr int A_BYTES = A_BOXES * NPL * WG_BOX_BYTES;
   static constexpr int W_BYTES = W_BOXES * NPL * WG_BOX_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
-  static constexpr int SCRATCH_BYTES = (WG_CONSUMER_THREADS / 32) * 2048;
-  static constexpr int RAW_STAGES = (227 * 1024 - 1024 - SCRATCH_BYTES - 2 * 8 * 8) / STAGE_BYTES;
-  static constexpr int NUM_STAGES = RAW_STAGES > 8 ? 8 : RAW_STAGES;
-  static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + SCRATCH_BYTES;
+  // next to the align slack, the barriers and the scratch
+  static constexpr int NUM_STAGES =
+      fd_tc_ring_stages(1024 + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES, STAGE_BYTES);
+  static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
   static_assert(NUM_STAGES >= 2, "pipeline needs at least two stages");
 };
 
 template <int BLOCK_N, int PREC, int NPL>
-__global__ void __launch_bounds__(WG_THREADS, 1)
+__global__ void __launch_bounds__(FD_TC_THREADS, 1)
 fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_constant__ CUtensorMap tm_row1,
                    const __grid_constant__ CUtensorMap tm_col0, const __grid_constant__ CUtensorMap tm_col1,
                    const FdWgradK p) {
@@ -63,18 +60,18 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   const int k_blocks = (p.T + WG_BLOCK_K - 1) / WG_BLOCK_K;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], WG_CONSUMER_THREADS / 32); }
+    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], FD_TC_CONSUMER_THREADS / 32); }
     fence_barrier_init();
   }
-  if (warp == WG_PRODUCER_WARP && lane == 0) {
+  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
     prefetch_tmap(&tm_row0); prefetch_tmap(&tm_row1); prefetch_tmap(&tm_col0); prefetch_tmap(&tm_col1);
   }
   __syncthreads();
 
-  if (warp >= WG_PRODUCER_WARP) {
+  if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
     producer_regs();
-    if (warp == WG_PRODUCER_WARP && lane == 0) {
+    if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         const int s = unit / tiles_per_split;
@@ -130,7 +127,7 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   consumer_regs();
   const int wg = warp / 4;                           // rows [64 wg, 64 wg + 64) of the tile = A box wg
   const int wq = warp % 4;
-  const uint32_t my_scratch = smem_u32(scratch_s) + warp * 2048;
+  const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
   const int j4 = (lane & 7) * 4, rsub = lane >> 3;
   // MN-major SW128 operands: LBO = distance between 64-channel atoms (the boxes), SBO = 8 time rows of 128 bytes
   constexpr uint32_t LBO = NPL * WG_BOX_BYTES, SBO = 1024;
@@ -198,47 +195,23 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   }
 }
 
-// planes [2][B][T][C] as a 4-D tensor (C, T, B, plane); box = [NPL planes][64 t][64 ch], 128-byte swizzle
-int make_plane_map(CUtensorMap* m, const uint16_t* ptr, int B, int T, int C, int npl) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  FD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)B, 2};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)T * C * 2, (cuuint64_t)B * T * C * 2};
-  cuuint32_t box[4] = {64, 64, 1, (cuuint32_t)npl};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<uint16_t*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  FD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(wgrad) failed: %d (B=%d T=%d C=%d ptr=%p)", (int)r, B, T, C,
-             (const void*)ptr);
-  return 0;
-}
-
-
+// row and column maps: box = [NPL planes][64 t][64 ch], 128-byte swizzle; absent second sources alias the first
 template <int BLOCK_N, int PREC, int NPL>
 int launch_wg(const FdWgradK& p, const uint16_t* const* row_ptr, const uint16_t* const* col_ptr, cudaStream_t stream) {
-  using C = WgCfg<BLOCK_N, NPL>;
   CUtensorMap tr[2], tc[2];
   for (int i = 0; i < 2; ++i) {
     const int ri = row_ptr[i] != nullptr ? i : 0, ci = col_ptr[i] != nullptr ? i : 0;
-    int rc = make_plane_map(&tr[i], row_ptr[ri], p.B, p.T, p.row_C[ri], NPL);
+    const long long rows_T = (long long)p.T * p.row_C[ri], cols_T = (long long)p.T * p.col_C[ci];
+    int rc = planes_map(&tr[i], row_ptr[ri], p.row_C[ri], p.T, p.B, p.row_C[ri], rows_T, p.B * rows_T, 64, WG_BLOCK_K,
+                        NPL, "wgrad rows");
     if (rc) return rc;
-    rc = make_plane_map(&tc[i], col_ptr[ci], p.B, p.T, p.col_C[ci], NPL);
+    rc = planes_map(&tc[i], col_ptr[ci], p.col_C[ci], p.T, p.B, p.col_C[ci], cols_T, p.B * cols_T, 64, WG_BLOCK_K, NPL,
+                    "wgrad columns");
     if (rc) return rc;
   }
-  auto kern = fd_wgrad_tc_kernel<BLOCK_N, PREC, NPL>;
-  static bool attr_set[FD_MAX_DEVICES] = {false};   // the max-dynamic-smem attribute is per device
-  const int dev = fd_current_device();
-  if (!attr_set[dev]) {
-    FD_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set[dev] = true;
-  }
-  const int g_wg_sms = fd_device_sms(dev);
-  const int units = p.splits * p.m_tiles * p.n_tiles;
-  const int grid = units < g_wg_sms ? units : g_wg_sms;
-  kern<<<grid, WG_THREADS, C::SMEM_BYTES, stream>>>(tr[0], tr[1], tc[0], tc[1], p);
-  FD_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return fd_tc_launch<fd_wgrad_tc_kernel<BLOCK_N, PREC, NPL>>(WgCfg<BLOCK_N, NPL>::SMEM_BYTES,
+                                                              p.splits * p.m_tiles * p.n_tiles, stream, false, tr[0],
+                                                              tr[1], tc[0], tc[1], p);
 }
 
 template <int BLOCK_N>
