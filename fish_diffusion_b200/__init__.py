@@ -12,6 +12,7 @@ from .diffusion import GaussianDiffusion, NaiveNoisePredictor, PLMSNoisePredicto
 from .nsf_hifigan import Generator, NsfHifiGAN  # noqa: F401
 from .mel import (MelSpectrogram, PitchAdjustableMelSpectrogram, dynamic_range_compression, get_mel_from_audio,  # noqa: F401
                   get_mel_transform)
+from .resample import resample, resample_length  # noqa: F401
 from .diffsinger import ENCODERS, DiffSinger, NaiveProjectionEncoder, load_checkpoint, pitch_to_scale  # noqa: F401
 from .fastspeech import FastSpeech2Encoder  # noqa: F401
 from .pipeline import BatchedSynthesizer, plan_batches  # noqa: F401

@@ -163,6 +163,8 @@ _SIGS = {
     "fd_stft_mag_eps_fwd": (c_int, [c_void_p] * 3 + [c_int, c_longlong, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
                                                      c_int, c_int, c_void_p]),
     "fd_log_clamp": (c_int, [c_void_p, c_void_p, c_longlong, c_float, c_float, c_void_p]),
+    "fd_resample_out_len": (c_longlong, [c_longlong, c_int, c_int]),
+    "fd_resample_fwd": (c_int, [c_void_p] * 6 + [c_int, c_longlong, c_longlong, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

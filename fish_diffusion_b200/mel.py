@@ -65,6 +65,58 @@ def dynamic_range_compression(x, C=1, clip_val=1e-5):
     return y
 
 
+# the parameters of librosa's default res_type "kaiser_best" (librosa 0.9.1 in the reference): a Kaiser-windowed sinc
+RESAMPLE_ZEROS = 64
+RESAMPLE_ROLLOFF = 0.9475937167399596
+RESAMPLE_BETA = 14.769656459379492
+_resample_banks = {}
+
+
+def resample_ratio(orig_sr, target_sr):
+    """-> (O, P): input / output samples per common period of the two integer rates."""
+    if int(orig_sr) != orig_sr or int(target_sr) != target_sr or orig_sr < 1 or target_sr < 1:
+        raise ValueError(f"sample rates must be positive integers, got {orig_sr!r} -> {target_sr!r}")
+    g = int(np.gcd(int(orig_sr), int(target_sr)))
+    return int(orig_sr) // g, int(target_sr) // g
+
+
+def kaiser_sinc_bank(orig_sr, target_sr):
+    """Polyphase filter bank of the resampler, float64 [P, 2W+O]: output q*P + p = sum_j h[p, j] * x[q*O - W + j].
+    One exact Kaiser-windowed sinc per output phase (no interpolated table): cutoff min(rates) * rolloff / 2,
+    RESAMPLE_ZEROS zero crossings each side, exactly zero from the last one on.  Also returns, per phase, the first
+    non-zero tap and the number of taps up to the last non-zero one (int32 [P]), and W."""
+    O, P = resample_ratio(orig_sr, target_sr)
+    base = min(O, P) * RESAMPLE_ROLLOFF                   # zero crossings per period
+    W = int(np.ceil(RESAMPLE_ZEROS * O / base))
+    num = (np.arange(2 * W + O, dtype=np.int64)[None, :] - W) * P - np.arange(P, dtype=np.int64)[:, None] * O
+    t = num.astype(np.float64) / (O * P) * base           # (input time - output time) in zero crossings
+    inside = np.abs(t) < RESAMPLE_ZEROS
+    win = np.i0(RESAMPLE_BETA * np.sqrt(np.where(inside, 1.0 - (t / RESAMPLE_ZEROS) ** 2, 0.0))) / np.i0(RESAMPLE_BETA)
+    h = np.where(inside, np.sinc(t) * win * (base / O), 0.0)
+    nz = h != 0.0
+    first = np.argmax(nz, axis=1)
+    count = h.shape[1] - np.argmax(nz[:, ::-1], axis=1) - first
+    return h, first.astype(np.int32), count.astype(np.int32), W
+
+
+def resample_bank(orig_sr, target_sr, device):
+    """The arguments of fd_resample_fwd, built once per (orig_sr, target_sr, device): kaiser_sinc_bank cast to fp32 and
+    laid out tap-major without the zero tails, bank[i, p] = h[p, first[p] + i] ([max count, P]); int32 first / count;
+    (O, P, W, taps)."""
+    key = (int(orig_sr), int(target_sr), str(device))
+    if key not in _resample_banks:
+        O, P = resample_ratio(orig_sr, target_sr)
+        if P * (2 * RESAMPLE_ZEROS * max(O, P) / min(O, P) + O) > 1 << 26:
+            raise ValueError(f"resample {orig_sr} -> {target_sr}: the rates share too small a common divisor "
+                             f"(O = {O}, P = {P}); the filter bank would hold more than 2**26 taps")
+        h, first, count, W = kaiser_sinc_bank(orig_sr, target_sr)
+        i = np.arange(int(count.max()))[:, None]
+        packed = np.where(i < count[None, :], h[np.arange(P)[None, :], np.minimum(first[None, :] + i, h.shape[1] - 1)], 0.0)
+        _resample_banks[key] = (torch.from_numpy(packed.astype(np.float32)).to(device), torch.from_numpy(first).to(device),
+                                torch.from_numpy(count).to(device), (O, P, W, h.shape[1]))
+    return _resample_banks[key]
+
+
 class PitchAdjustableMelSpectrogram:
     def __init__(self, sample_rate=44100, n_fft=2048, win_length=2048, hop_length=512, f_min=40, f_max=16000,
                  n_mels=128, center=False, precision="f16", backend="auto"):

@@ -24,6 +24,7 @@ from torch.nn.utils import remove_weight_norm, weight_norm
 from . import _native as N
 from .mel import PitchAdjustableMelSpectrogram, dynamic_range_compression
 from .registry import VOCODERS
+from .resample import resample
 
 LRELU_SLOPE = 0.1
 
@@ -536,9 +537,7 @@ class NsfHifiGAN(_Base):
         if sr is None:
             sr = self.h.sampling_rate
         if sr != self.h.sampling_rate:
-            import librosa  # resampling stays a host-side dependency exactly as in the reference
-            _w = librosa.resample(wav_torch.cpu().numpy(), orig_sr=sr, target_sr=self.h.sampling_rate)
-            wav_torch = torch.from_numpy(_w).to(wav_torch.device)
+            wav_torch = resample(wav_torch, sr, self.h.sampling_rate)   # on the device (librosa.resample in the reference)
         mel_torch = self.mel_transform(wav_torch, key_shift=key_shift, speed=speed)[0]
         mel_torch = dynamic_range_compression(mel_torch)
         if self.use_natural_log is False:

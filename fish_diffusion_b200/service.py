@@ -15,7 +15,16 @@ and concurrent requests are merged into ONE BatchedSynthesizer call per collecti
 buffers; here a single worker thread owns the model and the handler threads only queue work.
 
 ``frontend(audio float32 [n], sr, pitch_adjust, speaker_id) -> list of (features [T,E] CUDA, f0 [T] CUDA, n_samples)``
-``resample(audio, sr_in, sr_out) -> audio`` (identity when the rates match; the reference uses librosa.resample).
+``resample(audio, sr_in, sr_out) -> audio`` (identity when the rates match; the reference uses librosa.resample):
+pass ``device_resampler()``, the package's own Kaiser-sinc kernel.  The same kernel is the first stage of a ``frontend``
+whose content encoder wants 16 kHz audio (modules/feature_extractors/base.py:25)::
+
+    from fish_diffusion_b200 import resample
+    def frontend(audio, sr, pitch_adjust, speaker_id):
+        wav = torch.from_numpy(audio).cuda()[None]             # [1, n] at the model rate
+        wav16 = resample(wav, sr, 16000)                       # 44.1 k -> 16 k for HuBERT / ContentVec, on the device
+        ...
+    srv = make_http_server(worker, frontend, model_sr=44100, resample=device_resampler())
 """
 from __future__ import annotations
 
@@ -151,9 +160,29 @@ def _parse_multipart(body: bytes, content_type: str):
     return fields, files
 
 
+def device_resampler(device="cuda"):
+    """The ``resample=`` callable of make_http_server on the package's resampling kernel: (audio float32 [n] numpy,
+    sr_in, sr_out) -> float32 [ceil(n * sr_out / sr_in)] numpy.  Uploads, runs fd_resample_fwd, downloads; equal rates
+    pass the array through.  Replaces librosa.load(..., sr=model_sr) / librosa.resample(..., target_sr=daw_sample) of
+    flask_api.py:42,53."""
+    import torch
+    from .resample import resample
+
+    def run(audio, sr_in, sr_out):
+        audio = np.ascontiguousarray(audio, dtype=np.float32)
+        if int(sr_in) == int(sr_out) or audio.size == 0:
+            return audio
+        return resample(torch.from_numpy(audio).to(device), sr_in, sr_out).cpu().numpy()
+
+    return run
+
+
 def make_http_server(worker: BatchingWorker, frontend, host="0.0.0.0", port=6842, model_sr=44100,
                      resample: Optional[Callable] = None, default_speaker: Optional[int] = None):
-    """ThreadingHTTPServer with the reference's route (flask_api.py:24-60; port 6842 is what the VST plugin expects)."""
+    """ThreadingHTTPServer with the reference's route (flask_api.py:24-60; port 6842 is what the VST plugin expects).
+    `resample(audio, sr_in, sr_out)` converts the request to `model_sr` and the answer to the caller's `sampleRate`;
+    pass ``device_resampler()``.  The default None passes audio through unchanged, which is right only when the
+    caller's rate is the model's."""
     resample = resample or (lambda a, sr_in, sr_out: a)
 
     class Handler(BaseHTTPRequestHandler):
@@ -225,5 +254,5 @@ def unpack_frame(data: bytes) -> np.ndarray:
     return np.frombuffer(data, dtype=np.float32)
 
 
-__all__ = ["BatchingWorker", "convert", "make_http_server", "tcp_frame_loop", "wav_bytes", "read_wav", "pack_frame",
+__all__ = ["BatchingWorker", "convert", "device_resampler", "make_http_server", "tcp_frame_loop", "wav_bytes", "read_wav", "pack_frame",
            "unpack_frame"]

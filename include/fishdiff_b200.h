@@ -260,6 +260,23 @@ int fd_stft_mag_eps_fwd(const uint16_t* padded, const uint16_t* dft_w, uint16_t*
 /* log(clamp(x, clip)) * out_scale over fp32 (audio.py:11-18 dynamic_range_compression) */
 int fd_log_clamp(const float* x, float* y, long long n, float clip, float out_scale, void* stream);
 
+/* ------------------------------------------------------------------------------- resampling (a18) */
+/* Band-limited rational sample-rate conversion (librosa.resample on the host in the reference: nsf_hifigan.py:96,
+ * tools/diffusion/flask_api.py:42,53, modules/feature_extractors/base.py:25).  With g = gcd(sr_in, sr_out),
+ * O = sr_in/g, P = sr_out/g:   out[b][q*P + p] = sum_j h[p][j] * wav[b][q*O - W + j],   wav = 0 outside [0, lens[b]),
+ * h [P][taps = 2W + O] the polyphase filter (one low-pass per output phase; the caller designs it).
+ * n_out = fd_resample_out_len(n_in, sr_in, sr_out) = ceil(n_in*P/O) (librosa's and torchaudio's length rule); outputs
+ * past ceil(lens[b]*P/O) are written as zeros.  Negative on bad arguments. */
+long long fd_resample_out_len(long long n_in, int sr_in, int sr_out);
+/* wav [B][n_in] -> out [B][n_out]; per-phase first[P], count[P] (int32): phase p has its non-zero taps in
+ * [first[p], first[p] + count[p]) of its taps = 2W + O; bank [max count][P] fp32 holds them tap-major without the zero
+ * tails, bank[i][p] = h[p][first[p] + i] (a warp works on consecutive phases, so it reads one line per tap).
+ * lens [B] (int64, valid input samples per item) or NULL = n_in for all.  wav must be 16-byte aligned.
+ * The kernel stages 4*O + 2W samples or more in 48 KB of shared memory; ratios with a larger O are refused.
+ * Deterministic, no workspace: an item's result does not depend on the rest of the batch. */
+int fd_resample_fwd(const float* wav, const long long* lens, float* out, const float* bank, const int* first,
+                    const int* count, int B, long long n_in, long long n_out, int O, int P, int W, int taps, void* stream);
+
 /* ------------------------------------------------------------------ training step (a8): backward of the denoiser */
 /* General linear tap-GEMM: up to two source tensors [2][B][T][src_C], and a K offset w_kshift on the W operand (a
  * multiple of 8; selects a column block of W, e.g. the skip half of W2^T).  The data gradients of the WaveNet backward
