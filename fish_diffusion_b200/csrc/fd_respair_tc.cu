@@ -404,7 +404,7 @@ int launch_respair(const fd_respair_desc& d, FdResPairK p, cudaStream_t stream) 
   rc = planes_map(&tout_last, d.out_planes, C, p.T, p.B, rs, is, ps, K::BK_A, 128 - (p.k2 - 1), 1, "respair out_last");
   if (rc) return rc;
   const int tiles = p.B * ((p.T + p.r_out - 1) / p.r_out);
-  return fd_tc_launch<fd_respair_tc_kernel<C, PREC>>(FD_TC_SMEM_BUDGET, tiles, stream, true, tin, tw1, tw2, tout,
+  return fd_tc_launch<fd_respair_tc_kernel<C, PREC>>(FD_TC_SMEM_BUDGET, tiles, stream, true, 1, tin, tw1, tw2, tout,
                                                      tout_last, p);
 }
 

@@ -40,6 +40,35 @@ __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 
+// ---- thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the barrier at `bar`'s offset in CTA `cta` of the cluster.  CTA-scope release: a .release.cluster arrive
+// puts a MEMBAR.GPU in front of every call (DESIGN.md section 5)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n.reg .b32 ra;\nmapa.shared::cluster.u32 ra, %0, %1;\nmbarrier.arrive.shared::cluster.b64 _, [ra];\n}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+
+// named barrier ID (id 0 is __syncthreads) of N threads, a multiple of 32
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_arrive() {
+  asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -54,6 +83,17 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
       "r"(c2)
+      : "memory");
+}
+// the same box written at the same shared-memory offset of every CTA in `cta_mask`, completing bytes on the barrier at
+// the same offset in each of them
+__device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0,
+                                                      int c1, int c2, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6}], [%2], %3;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
+      "r"(c1), "r"(c2)
       : "memory");
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
@@ -574,23 +614,48 @@ int weights_map(CUtensorMap* m, const uint16_t* ptr, int N, int K, int box_k, in
   return encode_tiled(m, ptr, 3, dims, strides, box, what);
 }
 
-// Launches a persistent kernel of FD_TC_THREADS threads: one CTA per SM, at most one per work unit.  The dynamic
-// shared-memory limit is an attribute of each kernel and device, set on the kernel's first launch on a device (the
-// cache below is per Kern); `max_carveout` also asks for the largest shared-memory carveout.
+// Launches a persistent kernel of FD_TC_THREADS threads: one CTA per SM, at most one per work unit, in clusters of
+// `cluster` CTAs along x (the grid rounded down to a multiple of it, and capped at the clusters that fit on the device
+// at once, so that no cluster waits for another to finish).  The dynamic shared-memory limit is an attribute of each
+// kernel and device, set on the kernel's first launch on a device (the cache below is per Kern); `max_carveout` also
+// asks for the largest shared-memory carveout.
 template <auto Kern, typename... Args>
-int fd_tc_launch(int smem_bytes, int work_units, cudaStream_t stream, bool max_carveout, const Args&... args) {
+int fd_tc_launch(int smem_bytes, int work_units, cudaStream_t stream, bool max_carveout, int cluster,
+                 const Args&... args) {
   static bool attr_set[FD_MAX_DEVICES] = {false};
+  static int max_grid[FD_MAX_DEVICES];
   const int dev = fd_current_device();
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(FD_TC_THREADS);
+  cfg.dynamicSmemBytes = smem_bytes;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = cluster > 1 ? 1 : 0;
   if (!attr_set[dev]) {
     FD_CHECK_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     if (max_carveout)
       FD_CHECK_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributePreferredSharedMemoryCarveout,
                                          cudaSharedmemCarveoutMaxShared));
+    const int sms = fd_device_sms(dev);
+    max_grid[dev] = sms - sms % cluster;
+    if (cluster > 1) {
+      int clusters = 0;
+      cfg.gridDim = dim3(max_grid[dev]);
+      FD_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&clusters, Kern, &cfg));
+      FD_REQUIRE(clusters > 0, "no cluster of %d CTAs with %d bytes of shared memory fits on device %d", cluster,
+                 smem_bytes, dev);
+      if (clusters * cluster < max_grid[dev]) max_grid[dev] = clusters * cluster;
+    }
     attr_set[dev] = true;
   }
-  const int sms = fd_device_sms(dev);
-  Kern<<<work_units < sms ? work_units : sms, FD_TC_THREADS, smem_bytes, stream>>>(args...);
-  FD_CHECK_CUDA(cudaGetLastError());
+  const int grid = work_units < max_grid[dev] ? work_units : max_grid[dev];
+  cfg.gridDim = dim3(grid - grid % cluster);
+  FD_CHECK_CUDA(cudaLaunchKernelEx(&cfg, Kern, args...));
   return 0;
 }
 

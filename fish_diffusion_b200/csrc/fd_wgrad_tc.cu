@@ -210,7 +210,7 @@ int launch_wg(const FdWgradK& p, const uint16_t* const* row_ptr, const uint16_t*
     if (rc) return rc;
   }
   return fd_tc_launch<fd_wgrad_tc_kernel<BLOCK_N, PREC, NPL>>(WgCfg<BLOCK_N, NPL>::SMEM_BYTES,
-                                                              p.splits * p.m_tiles * p.n_tiles, stream, false, tr[0],
+                                                              p.splits * p.m_tiles * p.n_tiles, stream, false, 1, tr[0],
                                                               tr[1], tc[0], tc[1], p);
 }
 

@@ -4,11 +4,11 @@
     python tools/prof_wavenet_gemm.py [--single] [--reps N]
 
 Every dilation 1, 2, 4, 8 runs `reps` middle-layer blocks through fd_wavenet_block_fwd; each tap-GEMM launch is timed
-by its own CUDA-event pair (N.prof_enable / N.prof_collect).  Bytes staged per launch come from the tiling of
-fd_tapgemm_tc.cu: 128-row position tiles x 256-column tiles x 64-wide k-blocks, NPL operand planes each; the second
-figure is what would be staged if two CTAs on adjacent position tiles shared each W box (thread-block cluster pairs with
-a TMA multicast, see DESIGN.md section 5).  --single repeats the run in single-product mode (one hi*hi product, one plane
-staged)."""
+by its own CUDA-event pair (N.prof_enable / N.prof_collect).  Bytes per launch come from the ping-pong tiling of
+fd_tapgemm_tc.cu: 64-row position tiles x 256-column tiles, NPL operand planes each.  "staged" is what the TMA unit
+writes into shared memory (every CTA holds its own A box and the whole W box per 64 rows); "L2 read" is what it reads
+from L2 (the two CTAs of a cluster pair each fetch half of the W box and multicast it, so W is read once per 128 rows).
+--single repeats the run in single-product mode (one hi*hi product, one plane staged)."""
 import argparse
 import math
 import os
@@ -19,18 +19,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 B, T, C, E = 32, 4000, 512, 256
-BLOCK_M, BLOCK_N, BLOCK_K = 128, 256, 64
+BLOCK_M, BLOCK_N = 64, 256
 DILATIONS = (1, 2, 4, 8)
 
 
 def staged_bytes(k_total, npl):
-    """-> (bytes into shared memory per launch without multicast, with W shared by CTA pairs)."""
+    """-> (bytes written into shared memory per launch, bytes read from L2 per launch); independent of BLOCK_K."""
     m_tiles = B * math.ceil(T / BLOCK_M)
+    m_tiles += m_tiles % 2                     # an odd tile count leaves a pair half that still stages its W half
     tiles = m_tiles * (2 * C // BLOCK_N)
-    kb = k_total // BLOCK_K
-    a = BLOCK_M * BLOCK_K * 2 * npl
-    w = BLOCK_N * BLOCK_K * 2 * npl
-    return tiles * kb * (a + w), tiles * kb * (a + w / 2)
+    a = BLOCK_M * k_total * 2 * npl
+    w = BLOCK_N * k_total * 2 * npl
+    return tiles * (a + w), tiles * (a + w / 2)
 
 
 def gpu_info():
@@ -86,12 +86,12 @@ def run(N, torch, single, reps):
         ms = ms_sum / n
         alg = 2.0 * B * T * (2 * C) * k_total
         products = 1 if single else 3
-        plain, mcast = staged_bytes(k_total, npl)
+        staged, l2 = staged_bytes(k_total, npl)
         print(f"{name:15s} {ms:7.3f} ms/launch over {n} launches ({ms_sum / 1e3:.2f} s) | "
               f"{alg / ms / 1e9:6.1f} TFLOP/s alg, {products}x issued = "
-              f"{products * alg / ms / 1e9:6.1f} TFLOP/s | smem staged {plain / 1e9:5.2f} GB/launch "
-              f"({plain / ms / 1e9:5.2f} TB/s L2->SM), with W shared by CTA pairs {mcast / 1e9:5.2f} GB "
-              f"({mcast / ms / 1e9:5.2f} TB/s)", flush=True)
+              f"{products * alg / ms / 1e9:6.1f} TFLOP/s | smem staged {staged / 1e9:5.2f} GB/launch "
+              f"({staged / ms / 1e9:5.2f} TB/s into shared memory), L2 read {l2 / 1e9:5.2f} GB "
+              f"({l2 / ms / 1e9:5.2f} TB/s)", flush=True)
 
 
 def main():
