@@ -26,11 +26,11 @@ import torch
 
 from fish_diffusion_b200 import _native as N
 from gpu_util import dev
+from region_check import F64, Regions, pf64
 from wavenet_block_ref import gate_bias_tables, gate_bwd, gate_perm, gate_pre_packed, gate_z, res_skip
 
 pytestmark = pytest.mark.gpu
 
-F64 = torch.float64
 SKIP_SCALE = 1.0 / math.sqrt(20.0)
 
 # (rel-L2, max) bars per quantity and precision class, each <= 4x the worst value measured over the cases and back ends
@@ -73,54 +73,6 @@ TOL = {
 # single product against the FULL plane values: the half-precision rounding of both operands must show
 # (lower bound: it really is one product) and stay at that level (upper bound)
 X1_DEV = {"f16x1": (5e-5, 1e-3), "bf16x1": (5e-4, 8e-3)}   # measured 3.8e-4..4.0e-4 / 3.1e-3
-
-
-def pf64(planes, pc, hi_only=False):
-    """split planes int16 [2, ...] -> float64 hi + lo (or hi alone), on the planes' device"""
-    dt = torch.float16 if pc == N.PREC_F16 else torch.bfloat16
-    hi = planes[0].view(dt).to(F64)
-    return hi if hi_only else hi + planes[1].view(dt).to(F64)
-
-
-class Regions:
-    """Per-row-region error accumulation over item chunks: rows [0, dil), [T-dil, T), the last 128-row tile, the rest."""
-
-    def __init__(self, T, dil, device):
-        t = torch.arange(T, device=device)
-        lo, hi, last = t < dil, t >= T - dil, t >= (T - 1) // 128 * 128
-        self.masks = {"all": torch.ones_like(lo), "lo_edge": lo, "hi_edge": hi, "last_tile": last,
-                      "interior": ~(lo | hi | last)}
-        self.se = {k: 0.0 for k in self.masks}
-        self.sr = {k: 0.0 for k in self.masks}
-        self.mx = {k: 0.0 for k in self.masks}
-        self.n_all = 0
-
-    def add(self, got, ref):
-        """got / ref [b, T, n] float64"""
-        e = got - ref
-        for k, m in self.masks.items():
-            if not bool(m.any()):
-                continue
-            em, rm = e[:, m], ref[:, m]
-            self.se[k] += float((em * em).sum())
-            self.sr[k] += float((rm * rm).sum())
-            self.mx[k] = max(self.mx[k], float(em.abs().max()))
-        self.n_all += ref.numel()
-
-    def check(self, what, tol):
-        rtol, mtol = tol
-        rms = math.sqrt(self.sr["all"] / max(self.n_all, 1))
-        msgs, bad = [], []
-        for k in self.masks:
-            if self.sr[k] == 0.0 and self.se[k] == 0.0:
-                continue
-            rel = math.sqrt(self.se[k] / max(self.sr[k], 1e-300))
-            mx = self.mx[k] / max(rms, 1e-300)
-            msgs.append(f"{k} {rel:.2e}/{mx:.2e}")
-            if not (rel < rtol and mx < mtol):
-                bad.append(f"{k}: rel-L2 {rel:.2e} (bar {rtol:.1e}), max {mx:.2e} (bar {mtol:.1e})")
-        print(f"  {what}: " + ", ".join(msgs))
-        return [f"{what} {x}" for x in bad]
 
 
 def rel_l2(a, b):
