@@ -82,6 +82,7 @@ class WaveNetFwdDesc(ctypes.Structure):
         ("s", c_void_p), ("mlp_ws", c_void_p), ("gb", c_void_p), ("gb_ws", c_void_p),
         ("B", c_int), ("T", c_int), ("M", c_int), ("C", c_int), ("E", c_int), ("L", c_int), ("Bs", c_int),
         ("gate_tile", c_int), ("prec", c_int), ("backend", c_int),
+        ("cond_proj", c_void_p),
     ]
 
 
@@ -143,6 +144,7 @@ _SIGS = {
     "fd_wavenet_block_fwd": (c_int, [c_void_p] * 8 + [c_int, c_void_p, c_void_p, c_void_p, c_float] + [c_int] * 6 +
                              [c_float, c_float, c_int, c_int, c_int, c_void_p]),
     "fd_wavenet_fwd": (c_int, [POINTER(WaveNetFwdDesc), c_void_p]),
+    "fd_wavenet_cond_proj": (c_int, [POINTER(WaveNetFwdDesc), c_void_p]),
     "fd_conv_cl_fwd": (c_int, [POINTER(ConvDesc), c_void_p]),
     "fd_respair_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "fd_respair_fwd": (c_int, [POINTER(ResPairDesc), c_void_p]),

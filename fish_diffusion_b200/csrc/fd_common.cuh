@@ -81,8 +81,10 @@ struct FdTapGemm {
 
   // ---- FD_EPI_GATE (WaveNet GEMM1): column tile of width NT holds NT/2 gate columns followed by
   //      NT/2 filter columns for residual channels [tile*NT/2, (tile+1)*NT/2).
-  //      y = acc*acc_scale + gbias_full[n] - (t<dil ? gbias_lo[n] : 0) - (t+dil>=T ? gbias_hi[n] : 0)
+  //      y = acc*acc_scale + gbias_full[n] + addend[b,t,n] - (t<dil ? gbias_lo[n] : 0) - (t+dil>=T ? gbias_hi[n] : 0)
   //      z = sigmoid(y_gate) * tanh(y_filter)  -> out_planes [2][B][T][C]
+  //      addend (or null): fp32 [B][T][n_total] in the packed column order of W1 -- the conditioner projection computed
+  //      once per sampler call (fd_wavenet_cond_proj) when the GEMM runs the three tap segments only
   const float* gbias_full;  // [Bs][n_total]  (conv bias + cond bias + sum over 3 taps of W_tap.d)
   const float* gbias_lo;    // [Bs][n_total]  tap-0 (t-dil) contribution of the step vector
   const float* gbias_hi;    // [Bs][n_total]  tap-2 (t+dil) contribution
@@ -354,20 +356,27 @@ __device__ __forceinline__ void fd_epi_linear(const FdTapGemm& p, int b, int t, 
 }
 
 // gate epilogue: V gate accumulators + V filter accumulators for residual channels [zc0, zc0+V);
-// gb_* point at the bias of the FIRST gate column of this thread's chunk, gf_* at the first filter col.
+// *_g point at the bias of the FIRST gate column of this thread's chunk, *_f at the first filter col.
+// n_g / n_f: the packed columns of those two (for the addend).
 template <int V, int PREC = -1>
-__device__ __forceinline__ void fd_epi_gate(const FdTapGemm& p, int b, int t, int zc0,
+__device__ __forceinline__ void fd_epi_gate(const FdTapGemm& p, int b, int t, int zc0, int n_g, int n_f,
                                             const float (&g)[V], const float (&f)[V],
                                             const float* full_g, const float* full_f,
                                             const float* lo_g, const float* lo_f,
                                             const float* hi_g, const float* hi_f) {
   const int prec = PREC < 0 ? p.prec : PREC;   // compile-time in the tensor-core kernel
-  float z[V], yg8[V], yf8[V];
+  float z[V], yg8[V], yf8[V], ag[V], af[V];
   const bool e_lo = t < p.dil, e_hi = t + p.dil >= p.T;
+  if (p.addend != nullptr) {
+    const size_t arow = ((size_t)b * p.T + t) * p.n_total;
+    fd_load_f32<V>(p.addend + arow + n_g, ag);
+    fd_load_f32<V>(p.addend + arow + n_f, af);
+  }
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     float yg = g[i] * p.acc_scale + full_g[i];
     float yf = f[i] * p.acc_scale + full_f[i];
+    if (p.addend != nullptr) { yg += ag[i]; yf += af[i]; }
     if (e_lo) { yg -= lo_g[i]; yf -= lo_f[i]; }
     if (e_hi) { yg -= hi_g[i]; yf -= hi_f[i]; }
     yg8[i] = yg; yf8[i] = yf;

@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(256) fd_tapgemm_simt_kernel(const FdTapGemm p)
     } else if (EPI == FD_EPI_GATE) {
       if (n_a < p.n_total) {
         const size_t bo = (size_t)b * p.gbias_bstride;
-        fd_epi_gate<4>(p, b, t, j * RUN + tx * 4, v0, v1,
+        fd_epi_gate<4>(p, b, t, j * RUN + tx * 4, n_a, n_b, v0, v1,
                        p.gbias_full + bo + n_a, p.gbias_full + bo + n_b,
                        p.gbias_lo + bo + n_a, p.gbias_lo + bo + n_b,
                        p.gbias_hi + bo + n_a, p.gbias_hi + bo + n_b);

@@ -126,6 +126,16 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
           // `dilation` rows are skipped by a warp vote where no lane needs them
           float yg[8], yf[8], z[8];
           {
+            // the addend (conditioner projection, packed columns n0 + cc and n0 + HALF + cc of this row) is issued
+            // with the bias loads; it is read once per launch, so it streams past L2 (evict-first)
+            float4 c0, c1, d0, d1;
+            if (p.addend != nullptr) {
+              const float* ad = p.addend + yrow + n0 + cc;
+              c0 = __ldcs(reinterpret_cast<const float4*>(ad));
+              c1 = __ldcs(reinterpret_cast<const float4*>(ad + 4));
+              d0 = __ldcs(reinterpret_cast<const float4*>(ad + HALF));
+              d1 = __ldcs(reinterpret_cast<const float4*>(ad + HALF + 4));
+            }
             const float4 a0 = lds128(sb + 4u * cc), a1 = lds128(sb + 4u * cc + 16u);
             const float4 b0 = lds128(sb + 4u * (HALF + cc)), b1 = lds128(sb + 4u * (HALF + cc) + 16u);
             const float bg[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -134,6 +144,12 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
             for (int i = 0; i < 8; ++i) {
               yg[i] = g[i] * p.acc_scale + bg[i];
               yf[i] = f[i] * p.acc_scale + bf[i];
+            }
+            if (p.addend != nullptr) {
+              const float cg[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+              const float cf[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+#pragma unroll
+              for (int i = 0; i < 8; ++i) { yg[i] += cg[i]; yf[i] += cf[i]; }
             }
           }
           if (edge_any) {

@@ -3,8 +3,9 @@
 
 Same constructor, buffers (state_dict keys), attributes and ``forward`` / ``train_step`` contracts
 (diffusion.py:48-118,172-313; SURVEY.md section 8b), registered as ``DIFFUSIONS["GaussianDiffusion"]``.
-The sampler state lives channels-last on the device for the whole loop; the conditioner is split once per call;
-every update (DDPM posterior step, PLMS / UniPC linear combinations, norm/denorm) is one fused native kernel.
+The sampler state lives channels-last on the device for the whole loop; the conditioner is split once per call (and,
+with three GEMM products where it fits, projected for every layer once per call); every update (DDPM posterior step,
+PLMS / UniPC linear combinations, norm/denorm) is one fused native kernel.
 Scalar coefficient math stays on the host exactly like the reference's float32 buffers.
 """
 from __future__ import annotations
@@ -38,6 +39,19 @@ def get_noise_schedule_list(schedule_mode, timesteps, max_beta=0.01, s=0.008):
 
 
 to_torch = partial(torch.tensor, dtype=torch.float32)
+
+
+def hoist_cond_proj(denoiser, B: int, T: int, device) -> bool:
+    """Whether a sampler call keeps the conditioner projection of all layers resident and computes it once instead of
+    inside every GEMM1 launch.  Only with three tensor-core products: there the projection is a seventh of GEMM1's MMA
+    work; single-product GEMM1 gains less than the fp32 projection costs to read (at B=32, T=4000 the f16x1 sampler ran
+    3.34 s hoisted against 3.23 s fused, DESIGN.md section 5).  And only when the buffer takes at most a quarter of the
+    card's total memory (not of the free memory, which other processes on a shared GPU change from run to run), so a
+    given shape takes the same path every time."""
+    if N.mma_code(denoiser.precision) & N.PREC_SINGLE:
+        return False
+    nbytes = 4 * int(np.prod(denoiser.cond_proj_shape(B, T)))
+    return nbytes <= torch.cuda.mem_get_info(device)[1] // 4
 
 
 class NaiveNoisePredictor(nn.Module):
@@ -357,6 +371,16 @@ class GaussianDiffusion(nn.Module):
         elif cond_planes.data_ptr() != ws["cond_planes"].data_ptr():
             ws["cond_planes"].copy_(cond_planes)
             cond_planes = ws["cond_planes"]
+        # every evaluation of this call sees the same conditioner: its projection (all layers) is computed here, once
+        # per call and under the current weights, and GEMM1 then sums the conv taps only
+        cond_proj = None
+        if hoist_cond_proj(den, B, T, dev):
+            shape = den.cond_proj_shape(B, T)
+            if ws.get("cond_proj") is None or tuple(ws["cond_proj"].shape) != shape:
+                ws["cond_proj"] = torch.empty(shape, dtype=torch.float32, device=dev)
+            cond_proj = den.cond_projection(cond_planes, ws["cond_proj"])
+        else:
+            ws["cond_proj"] = None
         if original_mel is None:
             x = self._to_cl(x_T) if x_T is not None else self._randn((B, T, M), dev, out=ws["x"])
         else:
@@ -391,7 +415,8 @@ class GaussianDiffusion(nn.Module):
             steps = step_table.get(t_float)
             if steps is None:
                 steps = step_table[t_float] = torch.tensor([t_float], dtype=torch.float32, device=dev)
-            return den.forward_cl(xp, steps, cond_planes, x_mask=x_masks if masks else None, out=out)
+            return den.forward_cl(xp, steps, cond_planes, x_mask=x_masks if masks else None, out=out,
+                                  cond_proj=cond_proj)
 
         if noise_predictor in ("naive", "plms") and len(chunks) > 1:   # one upload for the whole schedule
             tab = torch.tensor([float(t) for t in chunks], dtype=torch.float32, device=dev)

@@ -331,12 +331,42 @@ class WaveNet(nn.Module):
         return WaveNetTrainFn.apply(self, masks, x_cl.contiguous(), cond_cl.contiguous(), d, *self.train_param_list())
 
     # ------------------------------------------------------------------------------------ native forward
+    def cond_proj_shape(self, B, T):
+        """Shape of the buffer cond_projection fills: [L, B, T, 2C] fp32 (L * 8C bytes per position)."""
+        return (self.n_layers, B, T, 2 * self.residual_channels)
+
     @torch.no_grad()
-    def forward_cl(self, x_planes, steps, cond_planes, x_mask=None, out=None):
+    def cond_projection(self, cond_planes, out):
+        """Every layer's conditioner_projection(conditioner) (wavenet.py:108) without its bias, for cond_planes
+        [2,B,T,E], into the caller-owned fp32 buffer `out` (cond_proj_shape) in W1's packed column order: L linear
+        tap-GEMMs over the conditioner columns of the current weight pack (fd_wavenet_cond_proj).  forward_cl(...,
+        cond_proj=out) then skips those columns in GEMM1; a sampler computes it once per call, since all its
+        evaluations share the conditioner.  Returns `out`."""
+        dev = cond_planes.device
+        N.require_cuda(cond_planes, "cond_planes")
+        _, B, T, E = cond_planes.shape
+        if E != self.d_encoder or tuple(out.shape) != self.cond_proj_shape(B, T) or out.dtype != torch.float32 \
+                or not out.is_contiguous() or out.device != dev:
+            raise ValueError(f"cond_projection: out must be contiguous float32 {self.cond_proj_shape(B, T)} on {dev}")
+        pk = self._packed(dev)                  # the current pack: a weight change since the last call is honoured
+        w1s = self._pack_static["w1"]
+        d = N.WaveNetFwdDesc()
+        d.cond_planes, d.cond_proj = N.ptr(cond_planes), N.ptr(out)
+        d.w1, d.w1_lstride = N.ptr(w1s), w1s.stride(0)
+        for l in range(self.n_layers):
+            d.w1_inv[l] = pk["w1_inv"][l]
+        d.B, d.T, d.C, d.E, d.L = B, T, self.residual_channels, E, self.n_layers
+        d.prec, d.backend = pk["mma"], pk["backend"]
+        N.check(N.lib().fd_wavenet_cond_proj(ctypes.byref(d), N.stream_ptr(dev)), "fd_wavenet_cond_proj")
+        return out
+
+    @torch.no_grad()
+    def forward_cl(self, x_planes, steps, cond_planes, x_mask=None, out=None, cond_proj=None):
         """Channels-last entry used by the fused sampler.
 
         x_planes [2,B,T,M] int16 split planes, steps float32 [1] or [B] (device), cond_planes [2,B,T,E],
-        x_mask uint8/bool [B,T] or None (True = masked).  Returns eps fp32 [B,T,M]."""
+        x_mask uint8/bool [B,T] or None (True = masked).  cond_proj: what cond_projection made of these cond_planes
+        under the current weights, or None (GEMM1 then projects the conditioner itself).  Returns eps fp32 [B,T,M]."""
         dev = x_planes.device
         N.require_cuda(x_planes, "x_planes")
         _, B, T, M = x_planes.shape
@@ -361,18 +391,21 @@ class WaveNet(nn.Module):
         # which also removes the per-launch tensor-map encodes from the host path.
         steps_buf = ws["steps"]
         steps_buf.copy_(steps, non_blocking=True)
+        if cond_proj is not None and tuple(cond_proj.shape) != self.cond_proj_shape(B, T):
+            raise ValueError(f"cond_proj must have shape {self.cond_proj_shape(B, T)}")
         d = self._fwd_desc(pk, ws, x_planes, cond_planes, steps_buf, x_mask, out, B, T, Bs)
+        d.cond_proj = N.ptr(cond_proj)
         use_graph = self.use_graph and not N.prof_is_on()
         if not use_graph:
             N.check(lib.fd_wavenet_fwd(ctypes.byref(d), st), "fd_wavenet_fwd")
             return out
         key = (x_planes.data_ptr(), cond_planes.data_ptr(), out.data_ptr(), 0 if x_mask is None else x_mask.data_ptr(),
-               B, T, Bs, self._pack_key, id(ws))
+               0 if cond_proj is None else cond_proj.data_ptr(), B, T, Bs, self._pack_key, id(ws))
         ent = self._graphs.get(key)
         if ent is None:                      # first sight of these buffers: run eagerly (lazy inits happen here)
             if len(self._graphs) >= 4:
                 self._graphs.clear()
-            self._graphs[key] = {"graph": None, "keep": (x_planes, cond_planes, out, x_mask, pk)}
+            self._graphs[key] = {"graph": None, "keep": (x_planes, cond_planes, out, x_mask, cond_proj, pk)}
             N.check(lib.fd_wavenet_fwd(ctypes.byref(d), st), "fd_wavenet_fwd")
             return out
         if ent["graph"] is None:

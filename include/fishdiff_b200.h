@@ -124,8 +124,19 @@ typedef struct fd_wavenet_fwd_desc {
   float* s; float* mlp_ws; float* gb; float* gb_ws;
   int B, T, M, C, E, L, Bs;
   int gate_tile, prec, backend;
+  /* conditioner projection of every layer (wavenet.py:108 `conditioner_projection(conditioner)`), fp32
+   * [L][B][T][2C] in the packed column order of w1, filled by fd_wavenet_cond_proj, or NULL.  Non-NULL: each layer's
+   * GEMM1 sums the three conv taps only and adds its [B][T][2C] slice in the gate epilogue (the sampler passes the
+   * same conditioner to every evaluation, so the projection is computed once per sampler call).  NULL: GEMM1 runs the
+   * conditioner columns itself. */
+  float* cond_proj;
 } fd_wavenet_fwd_desc;
 int fd_wavenet_fwd(const fd_wavenet_fwd_desc* d, void* stream);
+/* Fills d->cond_proj from d->cond_planes: L linear tap-GEMMs (K = E) that read the conditioner columns [3C, 3C+E) of
+ * each layer's packed w1 in place (acc_scale w1_inv[l]) and write fp32 without bias -- the conditioner bias stays in
+ * the gate-bias tables.  Uses cond_planes, w1, w1_lstride, w1_inv, B, T, C, E, L, prec, backend of the descriptor.
+ * B*T*2C must stay below 2^32. */
+int fd_wavenet_cond_proj(const fd_wavenet_fwd_desc* d, void* stream);
 
 /* One ResidualBlock.forward (wavenet.py:106-120), fused as two tap-GEMM launches:
  *   GEMM1  y = [W_conv(3 taps) | W_cond] . [x(t-d), x(t), x(t+d), cond(t)] + gate bias ; z = sigmoid(y_g)*tanh(y_f)

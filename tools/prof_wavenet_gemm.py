@@ -1,14 +1,18 @@
 """Per-launch device time of the two WaveNet tap-GEMMs (GEMM1 = GATE, GEMM2 = RES_SKIP) at the headline sampler shape
 (B=32, T=4000, C=512, E=256, f16), with the shared-memory traffic the tiling implies.
 
-    python tools/prof_wavenet_gemm.py [--single] [--reps N]
+    python tools/prof_wavenet_gemm.py [--single] [--hoisted] [--reps N]
 
 Every dilation 1, 2, 4, 8 runs `reps` middle-layer blocks through fd_wavenet_block_fwd; each tap-GEMM launch is timed
 by its own CUDA-event pair (N.prof_enable / N.prof_collect).  Bytes per launch come from the ping-pong tiling of
 fd_tapgemm_tc.cu: 64-row position tiles x 256-column tiles, NPL operand planes each.  "staged" is what the TMA unit
 writes into shared memory (every CTA holds its own A box and the whole W box per 64 rows); "L2 read" is what it reads
 from L2 (the two CTAs of a cluster pair each fetch half of the W box and multicast it, so W is read once per 128 rows).
---single repeats the run in single-product mode (one hi*hi product, one plane staged)."""
+--single repeats the run in single-product mode (one hi*hi product, one plane staged).
+--hoisted also times the sampler's path: the conditioner projection of all layers computed once per call
+(fd_wavenet_cond_proj, L linear tap-GEMMs with K = E; each launch timed) and GEMM1 over the three conv taps only
+(K = 3C) with the projection added in its epilogue, through fd_wavenet_fwd of a WaveNet with L = 4 layers
+(dilations 1, 2, 4, 8).  TFLOP/s are those of the K each launch actually sums."""
 import argparse
 import math
 import os
@@ -94,9 +98,58 @@ def run(N, torch, single, reps):
               f"({l2 / ms / 1e9:5.2f} TB/s)", flush=True)
 
 
+def run_hoisted(N, torch, single, reps):
+    from fish_diffusion_b200 import WaveNet, synthetic
+    dev = torch.device("cuda", 0)
+    M, L = 128, len(DILATIONS)
+    prec = "f16x1" if single else "f16"
+    cfg = dict(mel_channels=M, d_encoder=E, residual_channels=C, residual_layers=L, use_linear_bias=True)
+    net = WaveNet(**cfg, dilation_cycle=L, precision=prec, backend="tc").to(dev).eval()
+    net.load_state_dict({k: torch.from_numpy(v) for k, v in synthetic.wavenet_weights(0, **cfg).items()})
+    net.use_graph = False
+    pc = N.prec_code(prec)
+    g = torch.Generator(device=dev).manual_seed(0)
+    xp = N.split_nwc(torch.randn(B, T, M, device=dev, generator=g), pc)
+    cp = N.split_nwc(torch.randn(B, T, E, device=dev, generator=g), pc)
+    proj = torch.empty(net.cond_proj_shape(B, T), device=dev)
+    steps = torch.tensor([500.0], device=dev)
+    for _ in range(3):
+        net.cond_projection(cp, proj)
+        net.forward_cl(xp, steps, cp, cond_proj=proj)
+    torch.cuda.synchronize()
+    N.prof_enable(True)
+    for _ in range(reps):
+        net.cond_projection(cp, proj)
+    proj_prof, overflow = N.prof_collect()
+    for _ in range(reps):
+        net.forward_cl(xp, steps, cp, cond_proj=proj)
+    fwd_prof, overflow2 = N.prof_collect()
+    N.prof_enable(False)
+    assert not (overflow or overflow2), "per-launch event buffer overflowed: lower --reps"
+
+    products = 1 if single else 3
+    mode = "single product (hi*hi)" if single else "three products (lo*hi + hi*lo + hi*hi)"
+    print(f"== hoisted conditioner projection, {mode}, B={B} T={T} C={C} E={E}, dilations {DILATIONS} x {reps} calls")
+    proj_bytes = B * T * 2 * C * 4
+    rows = (("cond_proj linear", proj_prof["linear/tc"], E, "written"),
+            ("GEMM1 gate 3-seg", fwd_prof["gate/tc"], 3 * C, "read"))
+    for name, (ms_sum, n), k, how in rows:
+        ms = ms_sum / n
+        alg = 2.0 * B * T * (2 * C) * k
+        print(f"{name:17s} {ms:7.3f} ms/launch over {n} launches | {alg / ms / 1e9:6.1f} TFLOP/s alg (K={k}), "
+              f"{products}x issued = {products * alg / ms / 1e9:6.1f} TFLOP/s | fp32 projection {how} "
+              f"{proj_bytes / 1e9:5.2f} GB/launch ({proj_bytes / ms / 1e6:6.1f} GB/s)", flush=True)
+    ms_sum, n = fwd_prof["res_skip/tc"]
+    print(f"{'GEMM2 res_skip':17s} {ms_sum / n:7.3f} ms/launch over {n} launches", flush=True)
+    ms_sum, n = proj_prof["linear/tc"]
+    print(f"projection per sampler call of the 20-layer net: 20 x {ms_sum / n:.3f} = {20 * ms_sum / n:.2f} ms", flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--single", action="store_true", help="also run in single-product mode")
+    ap.add_argument("--hoisted", action="store_true",
+                    help="also time the projection hoisted out of GEMM1 (fd_wavenet_cond_proj + three-segment GATE)")
     ap.add_argument("--reps", type=int, default=200, help="blocks per dilation in the timed window")
     args = ap.parse_args()
     import torch
@@ -106,8 +159,12 @@ def main():
     assert torch.cuda.is_available(), "prof_wavenet_gemm.py needs a CUDA device"
     print(f"gpu: {gpu_info()} (name, power limit, max SM clock)")
     run(N, torch, False, args.reps)
+    if args.hoisted:
+        run_hoisted(N, torch, False, args.reps)
     if args.single:
         run(N, torch, True, args.reps)
+        if args.hoisted:
+            run_hoisted(N, torch, True, args.reps)
 
 
 if __name__ == "__main__":
