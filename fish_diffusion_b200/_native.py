@@ -20,7 +20,7 @@ PREC_F16, PREC_BF16 = 0, 1
 PREC_SINGLE = 0x10   # or-ed into the prec of GEMM calls: one product over the hi planes
 BACKEND_TC, BACKEND_SIMT = 0, 1
 ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class NativeError(RuntimeError):
@@ -93,7 +93,7 @@ class WaveNetBwdDesc(ctypes.Structure):
         ("dx_next", c_void_p), ("dskip", c_void_p), ("w2t", c_void_p), ("w1t", c_void_p), ("wct", c_void_p),
         ("w2t_inv", c_float), ("w1t_inv", c_float), ("wct_inv", c_float),
         ("dx_out", c_void_p), ("dx_f32", c_void_p), ("d_cond", c_void_p), ("gw1", c_void_p), ("gw2", c_void_p),
-        ("cs_dy", c_void_p), ("cs_edge", c_void_p), ("cs_dx", c_void_p), ("dz", c_void_p), ("dy", c_void_p),
+        ("cs_dy", c_void_p), ("cs_edge", c_void_p), ("cs_dx", c_void_p), ("dy", c_void_p),
         ("part1", c_void_p), ("part2", c_void_p), ("splits1", c_int), ("splits2", c_int),
         ("B", c_int), ("T", c_int), ("C", c_int), ("E", c_int), ("dilation", c_int), ("gate_tile", c_int),
         ("inv_S", c_float), ("prec", c_int), ("backend", c_int),
@@ -117,11 +117,9 @@ _SIGS = {
     "fd_wavenet_pack_layers": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "fd_wgrad_cl": (c_int, [POINTER(WgradDesc), c_void_p]),
     "fd_wavenet_block_bwd": (c_int, [POINTER(WaveNetBwdDesc), c_void_p]),
-    "fd_colsum_edges": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
     "fd_wavenet_block_fwd_train": (c_int, [c_void_p] * 10 + [c_int, c_void_p, c_void_p, c_void_p, c_float] +
                                    [c_int] * 6 + [c_float, c_float, c_int, c_int, c_int, c_void_p]),
     "fd_wavenet_gate_bias_from_d": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_void_p]),
-    "fd_gate_bwd": (c_int, [c_void_p] * 3 + [c_longlong, c_int, c_int, c_int, c_void_p]),
     "fd_relu_bwd": (c_int, [c_void_p] * 3 + [c_longlong, c_float, c_int, c_void_p]),
     "fd_lrelu_bwd": (c_int, [c_void_p] * 5 + [c_longlong, c_float, c_float, c_int, c_void_p]),
     "fd_colsum": (c_int, [c_void_p] * 3 + [c_int, c_int, c_int, c_float, c_int, c_void_p]),
@@ -344,8 +342,8 @@ def mrf_finish(ins, out, *, in_slope=0.1, scale=1.0, out_slope=0.1, prec=PREC_F1
 
 
 PROF_KINDS = {0: "linear/tc", 1: "linear/simt", 2: "gate/tc", 3: "gate/simt", 4: "res_skip/tc", 5: "res_skip/simt",
-              6: "mag/tc", 7: "mag/simt", 8: "gate_bwd/tc", 12: "respair/128", 13: "respair/64", 14: "respair/32",
-              15: "respair/16"}
+              6: "mag/tc", 7: "mag/simt", 8: "gate_bwd/tc", 9: "gate_bwd/simt", 12: "respair/128", 13: "respair/64",
+              14: "respair/32", 15: "respair/16"}
 
 
 _prof_on = False

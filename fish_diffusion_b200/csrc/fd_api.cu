@@ -369,9 +369,11 @@ int fd_gemm_cl_fwd(const fd_gemm_desc* d, void* stream) {
   p.epi = FD_EPI_LINEAR;
   p.bias = d->bias; p.bias_bstride = d->bias_bstride;
   if (d->gate_y != nullptr) {
-    FD_REQUIRE(d->backend == FD_BACKEND_TC, "fd_gemm_cl_fwd: the fused gate backward runs on the tensor-core back end only");
-    FD_REQUIRE(d->out_planes != nullptr && d->gate_tile > 0 && d->n_total % 4 == 0 && (d->gate_tile / 2) % 4 == 0,
-               "fd_gemm_cl_fwd: gate backward needs out_planes and a gate tile");
+    // whole 4-column groups on either side of a gate / filter split, and gate tiles that tile the 2C-wide dy / y rows
+    FD_REQUIRE(d->out_planes != nullptr && d->gate_tile > 0 && d->gate_tile % 8 == 0 && d->n_total % 4 == 0 &&
+                   d->n_total % (d->gate_tile / 2) == 0,
+               "fd_gemm_cl_fwd: gate backward needs out_planes and a gate tile (n_total=%d, gate_tile=%d)", d->n_total,
+               d->gate_tile);
   }
   p.addend = d->addend; p.res_f32 = d->res_f32; p.res_planes = d->res_planes; p.res_scale = d->res_scale;
   p.post_scale = d->post_scale; p.out_f32 = d->out_f32; p.out_accum = d->out_accum;

@@ -191,6 +191,13 @@ __device__ __forceinline__ float fd_tanh(float x) {
   return copysignf(r, x);
 }
 
+// backward of z = sigmoid(g) tanh(f) at one element: dz -> (dg, df); the GATE_BWD epilogue of both tap-GEMM kernels
+__device__ __forceinline__ void fd_dgate(float dz, float g, float f, float& dg, float& df) {
+  const float sg = fd_sigmoid(g), th = fd_tanh(f);
+  dg = dz * th * sg * (1.f - sg);
+  df = dz * sg * (1.f - th * th);
+}
+
 // ------------------------------------------------------------------------------------------------
 // vector helpers: V consecutive channels (V = 4 or 8)
 // ------------------------------------------------------------------------------------------------

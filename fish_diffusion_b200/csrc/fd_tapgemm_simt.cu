@@ -110,31 +110,82 @@ __global__ void __launch_bounds__(256) fd_tapgemm_simt_kernel(const FdTapGemm p)
   }
 
   // ---- epilogue
+  if constexpr (EPI == FD_EPI_GATE_BWD) {
+    // the accumulators are dz: dy of this thread's two 4-column groups, each gate group with its filter group half a
+    // tile further on, and the column sums of dy over this thread's rows
+    const int half = p.gate_tile / 2;
+    const size_t W2 = 2 * (size_t)p.C, plane = (size_t)p.B * p.T * W2;
+    const bool edge0 = t0 < p.dil, edge1 = t0 + BM + p.dil > p.T;   // CTA-uniform: the tile holds edge rows
 #pragma unroll
-  for (int r = 0; r < RM; ++r) {
-    const int t = t0 + ty * RM + r;
-    if (t >= p.T) continue;
-    float v0[4] = {acc[r][0], acc[r][1], acc[r][2], acc[r][3]};
-    float v1[4] = {acc[r][4], acc[r][5], acc[r][6], acc[r][7]};
-    const int n_a = run0 + tx * 4, n_b = run1 + tx * 4;
-    if (EPI == FD_EPI_LINEAR) {
-      const float* bias = p.bias ? p.bias + (size_t)b * p.bias_bstride : nullptr;
-      if (n_a < p.n_total) fd_epi_linear<4>(p, b, t, n_a, v0, bias, 0);
-      if (n_b < p.n_total) fd_epi_linear<4>(p, b, t, n_b, v1, bias, 0);
-    } else if (EPI == FD_EPI_GATE) {
-      if (n_a < p.n_total) {
-        const size_t bo = (size_t)b * p.gbias_bstride;
-        fd_epi_gate<4>(p, b, t, j * RUN + tx * 4, n_a, n_b, v0, v1,
-                       p.gbias_full + bo + n_a, p.gbias_full + bo + n_b,
-                       p.gbias_lo + bo + n_a, p.gbias_lo + bo + n_b,
-                       p.gbias_hi + bo + n_a, p.gbias_hi + bo + n_b);
+    for (int h = 0; h < 2; ++h) {
+      const int n = (h == 0 ? run0 : run1) + tx * 4;
+      const int pg = (n / half) * p.gate_tile + n % half;
+      float cs[8] = {}, e0[8] = {}, e1[8] = {};     // sums of dg (0..3) and df (4..7)
+#pragma unroll
+      for (int r = 0; r < RM; ++r) {
+        const int t = t0 + ty * RM + r;
+        if (t >= p.T || n >= p.n_total) continue;
+        const size_t off = ((size_t)b * p.T + t) * W2 + pg;
+        float g[4], f[4], dg[4], df[4];
+        fd_load_planes<4>(p.y_planes, plane, off, g, p.prec);
+        fd_load_planes<4>(p.y_planes, plane, off + half, f, p.prec);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) fd_dgate(acc[r][4 * h + i] * p.acc_scale, g[i], f[i], dg[i], df[i]);
+        fd_store_planes<4>(p.out_planes, plane, off, dg, p.prec);
+        fd_store_planes<4>(p.out_planes, plane, off + half, df, p.prec);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          cs[i] += dg[i]; cs[4 + i] += df[i];
+          if (t < p.dil) { e0[i] += dg[i]; e0[4 + i] += df[i]; }
+          if (t + p.dil >= p.T) { e1[i] += dg[i]; e1[4 + i] += df[i]; }
+        }
       }
-    } else if (EPI == FD_EPI_MAG) {
-      if (n_a < p.n_total) fd_epi_mag<4>(p, b, t, j * RUN + tx * 4, v0, v1);
-    } else {
-      const float* bias = p.bias + (size_t)b * p.bias_bstride;
-      if (n_a < p.n_total) fd_epi_res_skip<4>(p, b, t, n_a, v0, bias + n_a);
-      if (n_b < p.n_total) fd_epi_res_skip<4>(p, b, t, n_b, v1, bias + n_b);
+      // the lanes of a warp with this tx hold the same columns: sum over them, then one atomic per column and warp
+#pragma unroll
+      for (int o = TXC; o < 32; o *= 2)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          cs[i] += __shfl_xor_sync(0xffffffffu, cs[i], o);
+          if (edge0) e0[i] += __shfl_xor_sync(0xffffffffu, e0[i], o);
+          if (edge1) e1[i] += __shfl_xor_sync(0xffffffffu, e1[i], o);
+        }
+      if (tid % 32 >= TXC || n >= p.n_total) continue;
+      const size_t co = (size_t)b * W2 + pg;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const size_t c = co + (i < 4 ? i : half + i - 4);
+        if (p.cs != nullptr) atomicAdd(p.cs + c, cs[i] * p.cs_scale);
+        if (p.cs_edge != nullptr && edge0) atomicAdd(p.cs_edge + c, e0[i] * p.cs_scale);
+        if (p.cs_edge != nullptr && edge1) atomicAdd(p.cs_edge + (size_t)p.B * W2 + c, e1[i] * p.cs_scale);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < RM; ++r) {
+      const int t = t0 + ty * RM + r;
+      if (t >= p.T) continue;
+      float v0[4] = {acc[r][0], acc[r][1], acc[r][2], acc[r][3]};
+      float v1[4] = {acc[r][4], acc[r][5], acc[r][6], acc[r][7]};
+      const int n_a = run0 + tx * 4, n_b = run1 + tx * 4;
+      if (EPI == FD_EPI_LINEAR) {
+        const float* bias = p.bias ? p.bias + (size_t)b * p.bias_bstride : nullptr;
+        if (n_a < p.n_total) fd_epi_linear<4>(p, b, t, n_a, v0, bias, 0);
+        if (n_b < p.n_total) fd_epi_linear<4>(p, b, t, n_b, v1, bias, 0);
+      } else if (EPI == FD_EPI_GATE) {
+        if (n_a < p.n_total) {
+          const size_t bo = (size_t)b * p.gbias_bstride;
+          fd_epi_gate<4>(p, b, t, j * RUN + tx * 4, n_a, n_b, v0, v1,
+                         p.gbias_full + bo + n_a, p.gbias_full + bo + n_b,
+                         p.gbias_lo + bo + n_a, p.gbias_lo + bo + n_b,
+                         p.gbias_hi + bo + n_a, p.gbias_hi + bo + n_b);
+        }
+      } else if (EPI == FD_EPI_MAG) {
+        if (n_a < p.n_total) fd_epi_mag<4>(p, b, t, j * RUN + tx * 4, v0, v1);
+      } else {
+        const float* bias = p.bias + (size_t)b * p.bias_bstride;
+        if (n_a < p.n_total) fd_epi_res_skip<4>(p, b, t, n_a, v0, bias + n_a);
+        if (n_b < p.n_total) fd_epi_res_skip<4>(p, b, t, n_b, v1, bias + n_b);
+      }
     }
   }
 }
@@ -152,6 +203,9 @@ int launch_run(const FdTapGemm& p, cudaStream_t stream) {
   } else if (p.epi == FD_EPI_RES_SKIP) {
     grid.y = (p.n_total + 2 * RUN - 1) / (2 * RUN);
     fd_tapgemm_simt_kernel<RUN, FD_EPI_RES_SKIP><<<grid, block, 0, stream>>>(p);
+  } else if (p.epi == FD_EPI_GATE_BWD) {
+    grid.y = (p.n_total + 2 * RUN - 1) / (2 * RUN);
+    fd_tapgemm_simt_kernel<RUN, FD_EPI_GATE_BWD><<<grid, block, 0, stream>>>(p);
   } else {
     grid.y = (p.n_total + 2 * RUN - 1) / (2 * RUN);
     fd_tapgemm_simt_kernel<RUN, FD_EPI_LINEAR><<<grid, block, 0, stream>>>(p);

@@ -227,11 +227,7 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
           const float dzv[4] = {a[pp].x * p.acc_scale, a[pp].y * p.acc_scale, a[pp].z * p.acc_scale, a[pp].w * p.acc_scale};
           float dg[4], df[4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float sg = fd_sigmoid(g[i]), th = fd_tanh(f[i]);
-            dg[i] = dzv[i] * th * sg * (1.f - sg);
-            df[i] = dzv[i] * sg * (1.f - th * th);
-          }
+          for (int i = 0; i < 4; ++i) fd_dgate(dzv[i], g[i], f[i], dg[i], df[i]);
           uint32_t h0, l0, h1, l1;
           fd_split2(dg[0], dg[1], PREC, h0, l0);
           fd_split2(dg[2], dg[3], PREC, h1, l1);

@@ -9,34 +9,6 @@
 
 namespace {
 
-// dz (fp32 [rows][C]) and packed pre-activations y (planes [2][rows][2C]) -> dy planes [2][rows][2C] (packed order):
-//   z = sigmoid(g) tanh(f);  dg = dz * tanh(f) * sg (1 - sg);  df = dz * sg * (1 - tanh(f)^2)
-__global__ void k_gate_bwd(const float* __restrict__ dz, const uint16_t* __restrict__ y, uint16_t* __restrict__ dy,
-                           long long rows, int C, int gate_tile, int prec) {
-  const int half = gate_tile / 2;
-  const long long n4 = rows * C / 4;
-  const size_t plane = (size_t)rows * 2 * C;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-    const long long e = i * 4;
-    const long long row = e / C;
-    const int c = (int)(e % C);
-    const int ng = (c / half) * gate_tile + (c % half);
-    const size_t off = (size_t)row * 2 * C + ng;
-    float g[4], f[4], d4[4], dg[4], df[4];
-    fd_load_planes<4>(y, plane, off, g, prec);
-    fd_load_planes<4>(y, plane, off + half, f, prec);
-    fd_load_f32<4>(dz + e, d4);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float sg = fd_sigmoid(g[k]), th = fd_tanh(f[k]);
-      dg[k] = d4[k] * th * sg * (1.f - sg);
-      df[k] = d4[k] * sg * (1.f - th * th);
-    }
-    fd_store_planes<4>(dy, plane, off, dg, prec);
-    fd_store_planes<4>(dy, plane, off + half, df, prec);
-  }
-}
-
 // grad (fp32 [n]) masked by the sign of the forward activation (planes): out planes = split(grad * (act > 0) * scale)
 __global__ void k_relu_bwd(const float* __restrict__ grad, const uint16_t* __restrict__ act, uint16_t* __restrict__ out,
                            long long n, float scale, int prec) {
@@ -95,26 +67,6 @@ __global__ void k_colsum(const uint16_t* __restrict__ planes, const float* __res
   atomicAdd(out + (size_t)b * N + n, acc * scale);
 }
 
-// column sums over the first / last `e` time steps of every item: out[edge][b][n] += scale * sum in[b,t,n],
-// edge 0: t in [0,e), edge 1: t in [T-e,T)   (conv-tap edge corrections of the step-vector term in the weight gradient)
-__global__ void k_colsum_edges(const uint16_t* __restrict__ planes, float* __restrict__ out, int B, int T, int N, int e,
-                               float scale, int rows_per_block, int chunks, int prec) {
-  const int b = blockIdx.z;
-  const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= N) return;
-  const int edge = blockIdx.y / chunks, chunk = blockIdx.y % chunks;
-  const int base = edge == 0 ? 0 : T - e;
-  const int t0 = base + chunk * rows_per_block;
-  const int t1 = min(base + e, t0 + rows_per_block);
-  const size_t plane = (size_t)B * T * N;
-  float acc = 0.f;
-  for (int t = t0; t < t1; ++t) {
-    const size_t off = ((size_t)b * T + t) * N + n;
-    acc += fd_combine(planes[off], planes[plane + off], prec);
-  }
-  atomicAdd(out + ((size_t)edge * B + b) * N + n, acc * scale);
-}
-
 // out[i] = scale * sum_b in[b][i]
 __global__ void k_reduce_batch(const float* __restrict__ in, float* __restrict__ out, int B, long long n, float scale) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -132,15 +84,6 @@ inline int grid1d(long long work, int block = 256, int cap = 132 * 16) {
 }  // namespace
 
 extern "C" {
-
-int fd_gate_bwd(const float* dz, const uint16_t* y_planes, uint16_t* dy_planes, long long rows, int C, int gate_tile,
-                int prec, void* stream) {
-  FD_DEVICE_GUARD();
-  FD_REQUIRE(C % 4 == 0 && gate_tile % 8 == 0, "fd_gate_bwd: C=%d gate_tile=%d unsupported", C, gate_tile);
-  k_gate_bwd<<<grid1d(rows * C / 4), 256, 0, (cudaStream_t)stream>>>(dz, y_planes, dy_planes, rows, C, gate_tile, prec);
-  FD_LAUNCHED();
-  return 0;
-}
 
 int fd_relu_bwd(const float* grad, const uint16_t* act_planes, uint16_t* out_planes, long long n, float scale, int prec,
                 void* stream) {
@@ -174,19 +117,6 @@ int fd_colsum(const uint16_t* planes, const float* f32, float* out, int B, int T
   return 0;
 }
 
-int fd_colsum_edges(const uint16_t* planes, float* out, int B, int T, int N, int e, float scale, int prec,
-                    void* stream) {
-  FD_DEVICE_GUARD();
-  FD_REQUIRE(planes != nullptr && out != nullptr && e >= 0 && e <= T, "fd_colsum_edges: bad arguments (e=%d T=%d)", e, T);
-  if (e == 0) return 0;
-  const int rows_per_block = 64;
-  const int chunks = (e + rows_per_block - 1) / rows_per_block;
-  dim3 grid((N + 127) / 128, 2 * chunks, B);
-  k_colsum_edges<<<grid, 128, 0, (cudaStream_t)stream>>>(planes, out, B, T, N, e, scale, rows_per_block, chunks, prec);
-  FD_LAUNCHED();
-  return 0;
-}
-
 int fd_reduce_batch(const float* in, float* out, int B, long long n, float scale, void* stream) {
   FD_DEVICE_GUARD();
   k_reduce_batch<<<grid1d(n), 256, 0, (cudaStream_t)stream>>>(in, out, B, n, scale);
@@ -198,29 +128,23 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
   FD_DEVICE_GUARD();
   FD_REQUIRE(d != nullptr, "fd_wavenet_block_bwd: null descriptor");
   const int B = d->B, T = d->T, C = d->C, E = d->E, dil = d->dilation;
-  const bool tc = d->backend == FD_BACKEND_TC;
-  const int unit = tc ? 64 : 8;    // the tensor-core weight gradient takes 64-channel segments, its SIMT twin 8
+  // the tensor-core weight gradient takes 64-channel segments, its SIMT twin 8
+  const int unit = d->backend == FD_BACKEND_TC ? 64 : 8;
   FD_REQUIRE(B > 0 && T > 0 && C % unit == 0 && E % unit == 0 && dil > 0,
              "fd_wavenet_block_bwd: bad shape B=%d T=%d C=%d E=%d (backend %d)", B, T, C, E, d->backend);
   const float inv_sqrt2 = 0.70710678118654752440f;
-  const int edge = dil < T ? dil : T;
   int rc;
-  // ---- dy = gate backward of dz = [dx_next | d_skip] . W2 and the column sums of dy (K offset C selects the skip half
-  //      of W2^T when there is no residual gradient).  Tensor cores fuse the gate backward and the sums into the GEMM's
-  //      epilogue; the SIMT twin writes dz and runs them as separate kernels.
+  // ---- dy = gate backward of dz = [dx_next | d_skip] . W2 and the column sums of dy, both in the GEMM's epilogue (K
+  //      offset C selects the skip half of W2^T when there is no residual gradient)
   {
     fd_gemm_desc g;
     memset(&g, 0, sizeof(g));
     g.w = d->w2t; g.n_total = C; g.k_total = 2 * C; g.B = B; g.T = T;
     g.w_inv_scale = d->w2t_inv; g.res_scale = 1.f; g.post_scale = 1.f; g.planes_scale = 1.f;
     g.prec = d->prec; g.backend = d->backend;
-    if (tc) {
-      g.out_planes = d->dy;
-      g.gate_y = d->y_planes; g.gate_tile = d->gate_tile; g.gate_dil = edge;
-      g.gate_cs = d->cs_dy; g.gate_cs_edge = d->cs_edge; g.gate_cs_scale = d->inv_S;
-    } else {
-      g.out_f32 = d->dz;
-    }
+    g.out_planes = d->dy;
+    g.gate_y = d->y_planes; g.gate_tile = d->gate_tile; g.gate_dil = dil < T ? dil : T;
+    g.gate_cs = d->cs_dy; g.gate_cs_edge = d->cs_edge; g.gate_cs_scale = d->inv_S;
     if (d->dx_next == nullptr) {
       g.src[0] = d->dskip; g.src_C[0] = C; g.num_seg = 1; g.w_kshift = C;
       g.seg_src[0] = 0; g.seg_shift[0] = 0; g.seg_coff[0] = 0; g.seg_klen[0] = C;
@@ -230,15 +154,6 @@ int fd_wavenet_block_bwd(const fd_wavenet_bwd_desc* d, void* stream) {
     }
     rc = fd_gemm_cl_fwd(&g, stream);
     if (rc) return rc;
-    if (!tc) {
-      const int prec = d->prec & 0xF;
-      rc = fd_gate_bwd(d->dz, d->y_planes, d->dy, (long long)B * T, C, d->gate_tile, prec, stream);
-      if (rc) return rc;
-      rc = fd_colsum(d->dy, nullptr, d->cs_dy, B, T, 2 * C, d->inv_S, prec, stream);
-      if (rc) return rc;
-      rc = fd_colsum_edges(d->dy, d->cs_edge, B, T, 2 * C, edge, d->inv_S, prec, stream);
-      if (rc) return rc;
-    }
   }
   // ---- gw2 = [dx_next ; d_skip]^T . z
   {

@@ -4,7 +4,9 @@ inside GaussianDiffusion.p_losses, diffusion.py:129-151).
 
 Per residual block the backward is 5 GEMM launches (2x the forward FLOPs), issued by ONE native call
 (fd_wavenet_block_bwd) on either back end:
-  dz      = [dx_next/sqrt2 | d_skip] . W2                        data gradient of the output projection (K = 2C)
+  dz      = [dx_next/sqrt2 | d_skip] . W2                        data gradient of the output projection (K = 2C); its
+                                                                 epilogue turns dz into dy (gate backward) and the
+                                                                 column sums of dy, so dz is never stored
   dW2     = [dx_next/sqrt2 ; d_skip]^T . z                       weight gradient (K = time)
   dW1     = dy^T . [x(t-d)+d ; x(t)+d ; x(t+d)+d ; cond]         weight gradient of conv taps + conditioner, one GEMM
   dx      = sum_tap dy(t -/+ d) . W1_tap + dx_next/sqrt2         data gradient of the dilated conv (K = 6C)
@@ -194,7 +196,6 @@ class WaveNetTrainFn(torch.autograd.Function):
         cs_x = torch.zeros((L + 1, B, C), **f32)                             # colsum of d(x_l); row L stays zero
         gw1_all = torch.empty((L, 2 * C, KT), **f32)                         # packed row order, un-permuted at the end
         gw2_all = torch.empty((L, 2 * C, C), **f32)
-        dz = torch.empty((B, T, C), **f32)
         dx0 = torch.empty((B, T, C), **f32)       # fp32 copy of d(x_0), written by the layer-0 data gradient
         dy = torch.empty((2, B, T, 2 * C), **i16)
         dx_bufs = [torch.empty((2, B, T, C), **i16) for _ in range(2)]
@@ -205,7 +206,7 @@ class WaveNetTrainFn(torch.autograd.Function):
         part2 = torch.empty((splits2, 2 * C, C), **f32)
         bd = N.WaveNetBwdDesc()
         bd.cond_planes, bd.dskip = N.ptr(sv["cond_planes"]), N.ptr(dskip_planes)
-        bd.d_cond, bd.dz, bd.dy = N.ptr(d_cond), N.ptr(dz), N.ptr(dy)
+        bd.d_cond, bd.dy = N.ptr(d_cond), N.ptr(dy)
         bd.part1, bd.part2, bd.splits1, bd.splits2 = N.ptr(part1), N.ptr(part2), splits1, splits2
         bd.B, bd.T, bd.C, bd.E, bd.gate_tile = B, T, C, E, gate_tile
         bd.inv_S, bd.prec = inv_S, mma

@@ -32,7 +32,7 @@ extern "C" {
 #define FD_PREC_SINGLE 0x10
 #define FD_BACKEND_TC 0
 #define FD_BACKEND_SIMT 1
-#define FD_ABI_VERSION 2
+#define FD_ABI_VERSION 3
 
 /* ------------------------------------------------------------------------------------------- misc */
 int fd_abi_version(void);
@@ -47,7 +47,7 @@ void fd_set_device(int device);
 long long fd_launch_count(void);
 /* per-launch device timing of the tap-GEMM kernels (CUDA events on the launching stream), used by bench.py for
  * the roofline entry: kind = epilogue*2 + (backend==SIMT); epilogue 0 linear, 1 gate (WaveNet GEMM1),
- * 2 res/skip (WaveNet GEMM2), 3 DFT magnitude; kind 8 = gate backward fused into the dz GEMM; kinds 12..15 = fused ResBlock pair kernel at C = 128/64/32/16.  fd_prof_collect synchronises the device, fills ms_sum[k]/count[k]
+ * 2 res/skip (WaveNet GEMM2), 3 DFT magnitude, 4 gate backward fused into the dz GEMM; kinds 12..15 = fused ResBlock pair kernel at C = 128/64/32/16.  fd_prof_collect synchronises the device, fills ms_sum[k]/count[k]
  * for k < nkinds, resets the log and returns 1 if the log overflowed (65536 launches), 0 otherwise, <0 on error. */
 void fd_prof_enable(int on);
 int fd_prof_collect(double* ms_sum, long long* count, int nkinds);
@@ -311,11 +311,12 @@ typedef struct fd_gemm_desc {
   int out_accum, act, prec, backend;
   int bias_bstride;   /* 0: bias [n_total]; n_total: one bias vector per batch item, bias [B][n_total] (per-utterance
                          speaker / pitch-shift embeddings of DiffSinger.forward_features, diffsinger.py:95-121) */
-  /* gate backward fused into the epilogue (training; tensor-core back end only): when gate_y != NULL the accumulator is
+  /* gate backward fused into the epilogue (training, either back end): when gate_y != NULL the accumulator is
    * dz [B][T][n_total = C] and the epilogue writes dy = d(sigmoid(g) tanh(f)) (wavenet.py:113-115) for the saved
    * pre-activations gate_y [2][B][T][2C] (packed order of fd_wavenet_block_fwd_train) into out_planes [2][B][T][2C], and
    * adds gate_cs_scale * column sums of dy into gate_cs [B][2C] and -- over the first / last gate_dil steps of each item --
-   * gate_cs_edge [2][B][2C] (both zeroed by the caller; may be NULL).  Replaces fd_gate_bwd + fd_colsum + fd_colsum_edges. */
+   * gate_cs_edge [2][B][2C] (both zeroed by the caller; may be NULL).  gate_tile: a multiple of 8 whose half divides
+   * n_total. */
   const uint16_t* gate_y;
   float* gate_cs;
   float* gate_cs_edge;
@@ -336,9 +337,6 @@ int fd_wavenet_block_fwd_train(const uint16_t* x_planes, uint16_t* x_out_planes,
  * diffusion projections run under torch autograd on [Bs,C]-sized tensors) */
 int fd_wavenet_gate_bias_from_d(const float* d, const float* w1p, const float* bias_sum, float* gb_full, float* gb_lo,
                                 float* gb_hi, int L, int Bs, int C, int KT, void* stream);
-/* backward of z = sigmoid(g)*tanh(f) (wavenet.py:114-115): dz fp32 [rows][C], y planes [2][rows][2C] -> dy planes */
-int fd_gate_bwd(const float* dz, const uint16_t* y_planes, uint16_t* dy_planes, long long rows, int C, int gate_tile,
-                int prec, void* stream);
 /* out planes = split(grad * (act_planes > 0) * scale) (ReLU backward, wavenet.py:212,230) */
 int fd_relu_bwd(const float* grad, const uint16_t* act_planes, uint16_t* out_planes, long long n, float scale, int prec,
                 void* stream);
@@ -352,12 +350,6 @@ int fd_lrelu_bwd(const float* grad, const uint16_t* act_planes, const float* add
  * out must be zero-initialised by the caller */
 int fd_colsum(const uint16_t* planes, const float* f32, float* out, int B, int T, int N, float scale, int prec,
               void* stream);
-/* out[edge][b][n] += scale * sum_t planes[b,t,n] over t in [0,e) (edge 0) and [T-e,T) (edge 1); out zero-initialised
- * by the caller.  Autograd of `conv_layer(x + diffusion_step)` (modules/wavenet.py:107-111): the step vector d is added
- * before the zero-padded conv, so d(W_tap)/ += (sum over the steps where that tap reads inside [0,T) of dy) (x) d; the
- * sums are the full column sums minus these edge sums. */
-int fd_colsum_edges(const uint16_t* planes, float* out, int B, int T, int N, int e, float scale, int prec,
-                    void* stream);
 
 /* Weight gradient straight from channels-last split planes, no transposes:
  *   part[s][r][c] = acc_scale * sum_{b in split s} sum_t ROW[b,t,r] * COL[b,t+shift(c),c]
@@ -392,12 +384,12 @@ int fd_reduce_batch(const float* in, float* out, int B, long long n, float scale
 /* Backward of ONE ResidualBlock (autograd of modules/wavenet.py:106-120) as one native call: the 5 GEMM launches and the
  * elementwise / reduction kernels around them, issued back to back on `stream`:
  *   dz   = [dx_next/sqrt2 | d_skip] . W2            (fd_gemm_cl_fwd, two sources; skip half only above the last layer)
- *   dy   = gate backward of dz on the saved pre-activations (fused into the dz GEMM's epilogue on FD_BACKEND_TC;
- *          fd_gate_bwd, fd_colsum and fd_colsum_edges after a plain dz GEMM into the `dz` workspace on FD_BACKEND_SIMT)
+ *   dy   = gate backward of dz on the saved pre-activations (fused into the dz GEMM's epilogue, as are its column sums)
  *   gw2  = [dx_next ; d_skip]^T . z                  (fd_wgrad_cl + fd_reduce_batch; the 1/sqrt2 of the residual rows is
  *                                                     applied by the caller to all layers at once)
  *   gw1  = dy^T . [x(t-d) | x(t) | x(t+d) | cond]   (one weight-gradient GEMM, packed row order)
- *   cs_dy / cs_edge = column sums of dy (bias gradient, rank-one step-vector term of gw1)
+ *   cs_dy / cs_edge = column sums of dy over all steps / the first and last min(dilation, T) steps (bias gradient,
+ *                     rank-one step-vector term of gw1: the column sums minus the edge sums where a tap reads padding)
  *   dx   = conv^T(dy) + dx_next/sqrt2 -> planes (+ fp32 copy when dx_f32 != NULL);  d_cond += dy . Wc;  cs_dx = colsum(dx)
  * All gradients inside the chain carry the caller's power-of-two scale S; results that leave it are multiplied by
  * inv_S.  cs_dy [B][2C], cs_edge [2][B][2C], cs_dx [B][C] must be zero on entry.  part1 / part2: fp32 workspaces of
@@ -417,7 +409,7 @@ typedef struct fd_wavenet_bwd_desc {
   float* d_cond;               /* fp32 [B][T][E], accumulated, or NULL */
   float* gw1; float* gw2;      /* [2C][3C+E], [2C][C] */
   float* cs_dy; float* cs_edge; float* cs_dx;
-  float* dz; uint16_t* dy;     /* workspaces [B][T][C] fp32, [2][B][T][2C] planes */
+  uint16_t* dy;                /* workspace [2][B][T][2C] planes */
   float* part1; float* part2;
   int splits1, splits2;
   int B, T, C, E, dilation, gate_tile;

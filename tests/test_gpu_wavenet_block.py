@@ -4,7 +4,7 @@ to the oracle by test_wavenet_block_ref_cpu.py):
   * GEMM1 + GATE epilogue (dilated conv + conditioner + per-item or shared gate bias with its zero-padding
     corrections, z = sigmoid * tanh, pre-activations y in packed order when training),
   * GEMM2 + RES_SKIP epilogue (x' = (x + r)/sqrt2, skip accumulation, last-layer skip planes * skip_scale),
-  * the dz GEMM + GATE_BWD epilogue of the backward (dy, column sums and edge sums),
+  * the dz GEMM + GATE_BWD epilogue of the backward (dy, column sums and edge sums) on both back ends,
   * the gate-bias tables (fd_wavenet_gate_bias / _from_d).
 
 Every reference runs on the exact operand values the kernel read (split planes, fp32 bias tables), in torch float64
@@ -236,11 +236,16 @@ def test_block_forward_multi_tile_vs_float64(case):
 # ---------------------------------------------------------------------------------------------- gate backward
 # (name, C, gate_tile, precision, B, T, dil, two_segments)  --  gate_dil = min(dil, T) as fd_wavenet_block_bwd passes
 BWD = [
+    ("c80-f16-T77-d8-two", 80, 32, "f16", 3, 77, 8, True),                 # SIMT only (C not a multiple of 64)
+    ("c96-f16-T100-d17-two", 96, 32, "f16", 3, 100, 17, True),             # SIMT only: 2C = 192, 17-step edges
+    ("c128-bf16-T1-d8-one", 128, 256, "bf16", 3, 1, 8, False),             # T = 1: every row is in both edges
+    ("c192-f16-T129-d0-two", 192, 128, "f16", 2, 129, 0, True),            # gate_dil = 0: no edge rows
     ("c128-f16-T77-d8-two", 128, 256, "f16", 2, 77, 8, True),
     ("c128-bf16-T129-d200-one", 128, 256, "bf16", 3, 129, 200, False),     # gate_dil = T
     ("c192-f16-T200-d64-one", 192, 128, "f16", 2, 200, 64, False),
     ("c192-bf16-T129-d1-two", 192, 128, "bf16", 2, 129, 1, True),
     ("c512-f16-T1000-d64-two", 512, 256, "f16", 2, 1000, 64, True),
+    ("c512-f16-T300-d200-one", 512, 256, "f16", 2, 300, 200, False),       # ragged T < 2 dil over three row tiles
     ("c512-bf16-T77-d64-one", 512, 256, "bf16", 2, 77, 64, False),         # T < 2 dil
     ("c512-bf16x1-T300-d4-one", 512, 256, "bf16x1", 2, 300, 4, False),
     ("c512-f16-B32-T1000-d8-two", 512, 256, "f16", 32, 1000, 8, True),     # ~8 tiles per CTA
@@ -248,8 +253,13 @@ BWD = [
 ]
 
 
-@pytest.mark.parametrize("case", BWD, ids=[c[0] for c in BWD])
-def test_gate_bwd_epilogue_vs_float64(case):
+def _gate_bwd_params():
+    return [pytest.param(c, b, id=f"{c[0]}-{b}") for c in BWD
+            for b in (("tc", "simt") if c[1] % 64 == 0 else ("simt",))]
+
+
+@pytest.mark.parametrize("case,backend", _gate_bwd_params())
+def test_gate_bwd_epilogue_vs_float64(case, backend):
     name, C, gt, prec, B, T, dil, two = case
     pc, mma = N.prec_code(prec), N.mma_code(prec)
     hi = prec.endswith("x1")
@@ -277,7 +287,7 @@ def test_gate_bwd_epilogue_vs_float64(case):
     else:
         kw = dict(w_kshift=C)                             # the last layer: d_skip against the skip half of W2^T
         segs, src0 = [(0, 0, 0, C)], dsk
-    common = dict(w_inv_scale=1.0 / s, prec=mma, backend=N.BACKEND_TC, **kw)
+    common = dict(w_inv_scale=1.0 / s, prec=mma, backend=N.backend_code(backend), **kw)
     N.gemm_cl(src0, C, w2t, C, 2 * C, B, T, segs, out_f32=dz, **common)
     N.gemm_cl(src0, C, w2t, C, 2 * C, B, T, segs, out_planes=dy, gate_y=y, gate_tile=gt, gate_dil=gd, gate_cs=cs,
               gate_cs_edge=ce, gate_cs_scale=inv_S, **common)
@@ -288,7 +298,7 @@ def test_gate_bwd_epilogue_vs_float64(case):
     if two:
         dz_ref += pf64(dxn, pc, hi) @ wv[:, :C].T
     dy_ref = gate_bwd(dz_ref, pf64(y, pc), gt)   # the epilogue reads y at full plane precision in every mode
-    print(f"\n[{name}]")
+    print(f"\n[{name} {backend}]")
     bad = []
     for what, got, ref in (("dz", dz.to(F64), dz_ref), ("dy", pf64(dy, pc), dy_ref)):
         r = Regions(T, gd, d0)
@@ -299,6 +309,9 @@ def test_gate_bwd_epilogue_vs_float64(case):
             "cs_edge_hi": (ce[1], ce0[1], dy_ref[:, T - gd:].sum(1))}
     rtol, mtol = TOL[("cs", prec)]
     for what, (got, pre, ref) in sums.items():
+        if what != "cs" and gd == 0:
+            assert torch.equal(got, pre), f"{what}: gate_dil = 0 changed the edge sums"
+            continue
         inc, ref = got.to(F64) - pre.to(F64), ref * inv_S     # the prefill must be accumulated into, not overwritten
         rel = rel_l2(inc, ref)
         mx = float((inc - ref).abs().max()) / float(ref.pow(2).mean().sqrt())

@@ -72,16 +72,3 @@ def test_wgrad_direct_vs_float64(case, backend, prec, splits):
     e = rel_l2(got, ref)
     print(f"wgrad[{backend},{prec},B={B},T={T}] rel-L2 {e:.2e}")
     assert e < TOL[backend, pc], (e, np.abs(got - ref).max())
-
-
-def test_colsum_edges():
-    B, T, Nn, e = 3, 100, 192, 17
-    rng = np.random.RandomState(4)
-    a = torch.from_numpy(rng.randn(B, T, Nn).astype(np.float32)).to(dev())
-    pl = N.split_nwc(a, N.PREC_F16)
-    out = torch.zeros((2, B, Nn), dtype=torch.float32, device=dev())
-    N.check(N.lib().fd_colsum_edges(N.ptr(pl), N.ptr(out), B, T, Nn, e, 0.5, N.PREC_F16, N.stream_ptr(dev())),
-            "fd_colsum_edges")
-    v = planes_to_f64(pl, N.PREC_F16)
-    assert rel_l2(out[0].cpu().numpy(), 0.5 * v[:, :e].sum(1)) < 1e-6
-    assert rel_l2(out[1].cpu().numpy(), 0.5 * v[:, T - e:].sum(1)) < 1e-6

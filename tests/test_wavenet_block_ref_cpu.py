@@ -1,7 +1,8 @@
 """CPU tests behind test_gpu_wavenet_block.py, test_gpu_wavenet_block_bwd.py and test_gpu_wavenet_train_edges.py: the
 float64 block restatement equals the oracle's ResidualBlock, the closed forms of the block backward equal the autograd
-of that restatement, the whole-WaveNet restatement equals the oracle's, and the tensor-core launcher refuses a
-gate-backward GEMM whose 32-bit epilogue offsets would wrap."""
+of that restatement, the whole-WaveNet restatement equals the oracle's, the tensor-core launcher refuses a
+gate-backward GEMM whose 32-bit epilogue offsets would wrap, and fd_gemm_cl_fwd refuses a gate tile that does not tile
+the 2C-wide dy / y rows."""
 import ctypes
 import math
 
@@ -158,3 +159,26 @@ def test_gate_bwd_offset_guard():
     rc = N.lib().fd_gemm_cl_fwd(ctypes.byref(d), None)
     assert rc != 0
     assert "exceeds the 32-bit element offsets" in N.last_error(), N.last_error()
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="host-side check only: nothing may launch on these fake pointers")
+@pytest.mark.parametrize("backend", ["tc", "simt"])
+@pytest.mark.parametrize("C,gate_tile", [(192, 256), (80, 64), (128, 12)])
+def test_gate_bwd_gate_tile_guard(C, gate_tile, backend):
+    """The GATE_BWD epilogue reads y and writes dy at the packed gate column pg of a 4-column group and at pg + half:
+    a gate tile whose half does not divide n_total = C (C=192 with 256: pg + half runs to 2C + 64), or that is not a
+    multiple of 8, would reach past the 2C-wide rows and must be refused on either back end before any launch."""
+    from fish_diffusion_b200 import _native as N
+    B, T = 2, 16
+    d = N.GemmDesc()
+    fake = 1 << 40                                   # never dereferenced: the entry point must stop before the launch
+    d.src[0], d.src_C[0] = fake, C
+    d.w, d.n_total, d.k_total = fake, C, 2 * C
+    d.B, d.T, d.num_seg = B, T, 1
+    d.seg_src[0], d.seg_klen[0] = 0, C
+    d.out_planes, d.gate_y, d.gate_tile, d.gate_dil = fake, fake, gate_tile, 8
+    d.w_inv_scale, d.res_scale, d.post_scale, d.planes_scale = 1.0, 1.0, 1.0, 1.0
+    d.prec, d.backend = N.PREC_F16, N.backend_code(backend)
+    rc = N.lib().fd_gemm_cl_fwd(ctypes.byref(d), None)
+    assert rc != 0
+    assert "needs out_planes and a gate tile" in N.last_error(), N.last_error()
