@@ -20,6 +20,8 @@
 //     runs during the other's mainloop.  CTAs run in 2x1x1 clusters: the two CTAs of a pair work on adjacent 64-row
 //     tiles with the same column tile and each stages half of the W box into both (TMA multicast), so W is read from
 //     L2 once per 128 rows as in the cooperative schedule.
+//   The sampler's GATE (three products, conditioner projection in the epilogue) runs the ping-pong schedule with the
+//   operands swapped (fd_gate_t_kernel, "transposed GATE" below).
 // Pipeline: smem full/empty ring between the producer and the consumers.
 #include <cuda.h>
 #include "fd_common.cuh"
@@ -750,7 +752,285 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   cluster_sync();   // neither CTA leaves while the other may still multicast into it or arrive on its barriers
 }
 
+// ------------------------------------------------------------------ transposed GATE (the sampler's GEMM1)
+// GEMM1 with the conditioner projection hoisted out (three conv taps of the residual stream, K = 3C, the projection
+// added in the epilogue) and three products, with the operands swapped: 64 packed W1 rows are the wgmma M side and
+// BLOCK_T time steps the N side.  A stage holds one 32-channel block: the activation rows [t0 - d, t0 + BLOCK_T + d)
+// once, and the three taps' W boxes.  Tap j reads the activation tile from row j d on -- a descriptor start address
+// moved by j d rows (see make_smem_desc) -- so each activation row is staged once for all three taps instead of once
+// per tap, and the W box per stage is 64 rows instead of 256.
+// The W tensor map views the existing pack (tiles of gate_tile rows: gate_tile / 2 gates, then their filters) as
+// (K, 8 rows, gate | filter, 8-row group, plane): a box lands as 16-row groups of 8 gate rows followed by the 8
+// matching filter rows, so a thread's accumulator rows r and r + 8 are the gate and the filter of one channel and the
+// gate needs no exchange between threads.  The bias tables and the conditioner projection keep W1's packed order.
+// Schedule: that of fd_tapgemm_pp_kernel (ping-pong warpgroups, 2x1x1 clusters); a work unit is (time tile, pair of
+// adjacent 64-row W tiles), CTA `rank` of the pair computes W tile 2 pair + rank, and each CTA multicasts one plane of
+// the shared activation tile into both.
+template <int BLOCK_T>
+struct GateTCfg {
+  static constexpr int BLOCK_K = 32;                      // 64-byte rows: a 64-wide ring would hold 2 stages
+  static constexpr int ROW_BYTES = BLOCK_K * 2;
+  static constexpr int ACT_ROWS = BLOCK_T + 16;           // the halo: dilations up to MAX_DIL
+  static constexpr int MAX_DIL = (ACT_ROWS - BLOCK_T) / 2;
+  static constexpr int ACT_PLANE = ACT_ROWS * ROW_BYTES;
+  static constexpr int W_PLANE = 64 * ROW_BYTES;
+  static constexpr int W_OFF = 2 * ACT_PLANE;             // then tap j's W box (hi plane, lo plane) at W_OFF + 2 j W_PLANE
+  static constexpr int STAGE_BYTES = W_OFF + 3 * 2 * W_PLANE;
+  static constexpr uint32_t SWIZZLE_MODE = swizzle_mode_for(ROW_BYTES);
+  static constexpr uint32_t SBO = 8 * ROW_BYTES;
+  static constexpr int NUM_STAGES =
+      fd_tc_ring_stages(1024 /*align slack*/ + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES, STAGE_BYTES);
+  static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
+  static_assert(ACT_ROWS <= 256, "one TMA box per plane");
+  static_assert(ACT_PLANE % 512 == 0 && STAGE_BYTES % 1024 == 0, "planes start on 64 B swizzle atoms");
+  static_assert(NUM_STAGES >= 3, "ring depth");
+  static_assert(SMEM_BYTES <= FD_TC_SMEM_BUDGET, "shared memory");
+};
+
+// Epilogue of one warp: rows [16 wq, 16 wq + 16) of the tile are residual channels ch .. ch + 7 (gates, then
+// filters); lane -> channel ch + lane / 4, times t0 + 8 c + 2 (lane % 4) + {0, 1}.  z goes through the warp's scratch,
+// 32 time steps at a time, so that each lane stores the 8 channels of one time step (16 bytes per plane).
+template <int BLOCK_T, int PREC>
+__device__ __forceinline__ void gate_t_epilogue(const FdTapGemm& p, const float* acc, int b, int t0, int ch,
+                                                uint32_t my_scratch, int lane) {
+  const int half = p.gate_tile / 2;
+  const int e = lane >> 2, q4 = lane & 3;
+  const int n_g = (ch / half) * p.gate_tile + ch % half + e, n_f = n_g + half;   // packed columns of rows r, r + 8
+  const size_t bo = (size_t)b * p.gbias_bstride;
+  const float bg = p.gbias_full[bo + n_g], bf = p.gbias_full[bo + n_f];
+  const float lg = p.gbias_lo[bo + n_g], lf = p.gbias_lo[bo + n_f];
+  const float hg = p.gbias_hi[bo + n_g], hf = p.gbias_hi[bo + n_f];
+  const size_t row0 = (size_t)b * p.T;
+  const size_t zplane = (size_t)p.B * p.T * p.C;
+  constexpr int NG = BLOCK_T / 8;                          // 8-column groups of the fragment
+  // The addend (read once per launch: it streams past L2, evict-first) of a 32-step chunk, (gate, filter) per step,
+  // rows past T clamped.  The loads of chunk c + 1 are issued before chunk c is computed: issued next to their use,
+  // each would wait out a DRAM round trip, and the epilogue would outlast the other warpgroup's mainloop.
+  auto load_addend = [&](int c0, float (&a)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) a[i] = 0.f;
+    if (p.addend == nullptr) return;
+#pragma unroll
+    for (int ci = 0; ci < 4; ++ci) {
+      if (c0 + ci < NG) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const int t = min(t0 + 8 * (c0 + ci) + 2 * q4 + s, p.T - 1);
+          const float* ad = p.addend + (row0 + t) * p.n_total;
+          a[4 * ci + 2 * s] = __ldcs(ad + n_g);
+          a[4 * ci + 2 * s + 1] = __ldcs(ad + n_f);
+        }
+      }
+    }
+  };
+  float a_next[16];
+  load_addend(0, a_next);
+#pragma unroll
+  for (int c0 = 0; c0 < NG; c0 += 4) {
+    float a_cur[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) a_cur[i] = a_next[i];
+    if (c0 + 4 < NG) load_addend(c0 + 4, a_next);
+#pragma unroll
+    for (int ci = 0; ci < 4; ++ci) {
+      if (c0 + ci < NG) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const int tl = 8 * ci + 2 * q4 + s;              // time step inside the 32-step chunk
+          const int t = t0 + 8 * c0 + tl;
+          float yg = acc[4 * (c0 + ci) + s] * p.acc_scale + bg + a_cur[4 * ci + 2 * s];
+          float yf = acc[4 * (c0 + ci) + 2 + s] * p.acc_scale + bf + a_cur[4 * ci + 2 * s + 1];
+          if (t < p.dil) { yg -= lg; yf -= lf; }
+          if (t + p.dil >= p.T) { yg -= hg; yf -= hf; }
+          // scratch [32 steps][8 channels], the two 16-byte halves of a step swapped on every other group of 4 steps
+          sts32(my_scratch + 4u * (tl * 8 + (((e >> 2) ^ ((tl >> 2) & 1)) << 2) + (e & 3)),
+                fd_sigmoid(yg) * fd_tanh(yf));
+        }
+      }
+    }
+    __syncwarp();
+    const int t = t0 + 8 * c0 + lane;
+    if (lane < 8 * min(4, NG - c0) && t < p.T) {
+      const uint32_t sw = (uint32_t)((lane >> 2) & 1);
+      const float4 z0 = lds128(my_scratch + 4u * (lane * 8 + (sw << 2)));
+      const float4 z1 = lds128(my_scratch + 4u * (lane * 8 + ((sw ^ 1u) << 2)));
+      const float z[8] = {z0.x, z0.y, z0.z, z0.w, z1.x, z1.y, z1.z, z1.w};
+      fd_store_planes<8>(p.out_planes, zplane, (row0 + t) * p.C + ch, z, PREC);
+    }
+    __syncwarp();
+  }
+}
+
+template <int BLOCK_T, int PREC>
+__global__ void __launch_bounds__(FD_TC_THREADS, 1)
+fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const FdTapGemm p) {
+  using C = GateTCfg<BLOCK_T>;
+  using MMA = Wgmma<BLOCK_T, PREC>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* stage_base = smem;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::NUM_STAGES * C::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + C::NUM_STAGES;
+  float* scratch_s = reinterpret_cast<float*>(empty_bar + C::NUM_STAGES);
+
+  const int warp = threadIdx.x / 32;
+  const int lane = threadIdx.x % 32;
+  const int rank = (int)cluster_ctarank();
+  const int pair = blockIdx.x / 2, num_pairs = gridDim.x / 2;
+
+  const int d = p.dil;
+  const int tiles_t = (p.T + BLOCK_T - 1) / BLOCK_T;
+  const int num_wp = p.n_total / 128;                      // pairs of 64-row W tiles
+  const int num_units = p.B * tiles_t * num_wp;
+  const int k_blocks = p.C / C::BLOCK_K;
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * 4); }
+    fence_barrier_init();
+  }
+  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
+    prefetch_tmap(&tm_x);
+    prefetch_tmap(&tm_w);
+  }
+  cluster_sync();
+
+  if (warp >= FD_TC_PRODUCER_WARP) {
+    // =========================================================== TMA producer
+    producer_regs();
+    if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
+      // both activation planes (one from each CTA of the pair) + this CTA's three W boxes
+      const uint32_t tx = 2u * (uint32_t)(BLOCK_T + 2 * d) * C::ROW_BYTES + 3 * 2 * C::W_PLANE;
+      const int half = p.gate_tile / 2;
+      int stage = 0; uint32_t phase = 0;
+      for (int u = pair; u < num_units; u += num_pairs) {
+        const int tt = u / num_wp, wt = 2 * (u % num_wp) + rank;
+        const int b = tt / tiles_t, t0 = (tt % tiles_t) * BLOCK_T;
+        const int ch = wt * 32;                                         // first residual channel of the W tile
+        const int g0 = ((ch / half) * p.gate_tile + ch % half) / 8;     // its first 8-row group of gate rows
+#pragma unroll 1
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* st = stage_base + stage * C::STAGE_BYTES;
+          mbar_expect_tx(&full_bar[stage], tx);
+          tma_load_4d_multicast(st + rank * C::ACT_PLANE, &tm_x, &full_bar[stage], kb * C::BLOCK_K, t0 - d, b, rank,
+                                0x3);
+#pragma unroll 1
+          for (int j = 0; j < 3; ++j)
+            tma_load_5d(st + C::W_OFF + j * 2 * C::W_PLANE, &tm_w, &full_bar[stage], j * p.C + kb * C::BLOCK_K, 0, 0,
+                        g0, 0);
+          if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // =========================================================== consumers: one warpgroup per unit, in turn
+    consumer_regs();
+    const int wg = warp / 4;
+    const int wq = warp % 4;
+    const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
+    float acc[BLOCK_T / 2];
+    int stage = 0; uint32_t phase = 0;
+    auto advance = [&](int n) {
+      stage += n;
+      phase ^= (uint32_t)(stage / C::NUM_STAGES) & 1u;
+      stage %= C::NUM_STAGES;
+    };
+    auto release = [&](int st) {
+      if (lane == 0) { mbar_arrive_cluster(&empty_bar[st], 0); mbar_arrive_cluster(&empty_bar[st], 1); }
+    };
+    if (wg == 1) advance(k_blocks);
+    for (int u = pair + wg * num_pairs; u < num_units; u += 2 * num_pairs) {
+      const int tt = u / num_wp, wt = 2 * (u % num_wp) + rank;
+      const int b = tt / tiles_t, t0 = (tt % tiles_t) * BLOCK_T;
+
+      if (u != pair) wg == 0 ? named_bar_sync<1, 256>() : named_bar_sync<2, 256>();   // wait for the turn
+      const bool pass = u + num_pairs < num_units;
+#pragma unroll
+      for (int i = 0; i < BLOCK_T / 2; ++i) acc[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        wg_fence_operand(acc);
+        wg_fence();
+        const uint32_t st = smem_u32(stage_base + stage * C::STAGE_BYTES);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          const uint32_t xa = st + (uint32_t)(j * d * C::ROW_BYTES);       // tap j: activation rows t0 - d + j d ...
+          const uint64_t x_hi = make_smem_desc(xa, 16, C::SBO, C::SWIZZLE_MODE);
+          const uint64_t x_lo = make_smem_desc(xa + C::ACT_PLANE, 16, C::SBO, C::SWIZZLE_MODE);
+          const uint32_t wa = st + C::W_OFF + j * 2 * C::W_PLANE;
+          const uint64_t w_hi = make_smem_desc(wa, 16, C::SBO, C::SWIZZLE_MODE);
+          const uint64_t w_lo = make_smem_desc(wa + C::W_PLANE, 16, C::SBO, C::SWIZZLE_MODE);
+#pragma unroll
+          for (int k = 0; k < C::BLOCK_K / 16; ++k) {
+            const uint64_t adv = (uint64_t)((k * 32) >> 4);
+            // the products in the order of the other orientation: small terms first, hi*hi last
+            MMA::template ss<0, 0>(acc, w_hi + adv, x_lo + adv, 1u);
+            MMA::template ss<0, 0>(acc, w_lo + adv, x_hi + adv, 1u);
+            MMA::template ss<0, 0>(acc, w_hi + adv, x_hi + adv, 1u);
+          }
+        }
+        wg_commit();
+        if (kb == k_blocks - 1 && pass) wg == 0 ? named_bar_arrive<2, 256>() : named_bar_arrive<1, 256>();
+        wg_wait<1>();
+        wg_fence_operand(acc);
+        if (prev_stage >= 0) release(prev_stage);
+        prev_stage = stage;
+        advance(1);
+      }
+      wg_wait<0>();
+      wg_fence_operand(acc);
+      if (prev_stage >= 0) release(prev_stage);
+      advance(k_blocks);
+
+      gate_t_epilogue<BLOCK_T, PREC>(p, acc, b, t0, wt * 32 + wq * 8, my_scratch, lane);
+    }
+  }
+  __syncwarp();
+  cluster_sync();
+}
+
 // ------------------------------------------------------------------ host side
+// The transposed GATE's time-tile width for p, or 0 where it does not apply (the other GEMMs, training's forward,
+// which keeps the pre-activations, the conditioner in the K loop, one product, a halo past MAX_DIL): of the
+// instantiated widths, the one that pads T least.
+int gate_t_block(const FdTapGemm& p) {
+  if (p.epi != FD_EPI_GATE || p.single || p.y_planes != nullptr || p.num_seg != 3 || p.w_kshift != 0) return 0;
+  if (p.C % GateTCfg<200>::BLOCK_K != 0 || p.n_total != 2 * p.C || p.src_C[0] != p.C) return 0;
+  if ((p.gate_tile != 256 && p.gate_tile != 128) || p.n_total % p.gate_tile != 0) return 0;
+  for (int s = 0; s < 3; ++s)
+    if (p.seg[s].src != 0 || p.seg[s].shift != (s - 1) * p.dil || p.seg[s].c_off != 0 || p.seg[s].k_len != p.C)
+      return 0;
+  int best = 0;
+  long long best_pad = 0;
+  for (const int bt : {200, 240}) {
+    if (p.dil > (bt == 200 ? GateTCfg<200>::MAX_DIL : GateTCfg<240>::MAX_DIL)) continue;
+    const long long pad = (long long)(p.T + bt - 1) / bt * bt;
+    if (best == 0 || pad < best_pad || (pad == best_pad && bt > best)) { best = bt; best_pad = pad; }
+  }
+  return best;
+}
+
+template <int BLOCK_T, int PREC>
+int launch_gate_t(const FdTapGemm& p, cudaStream_t stream) {
+  using C = GateTCfg<BLOCK_T>;
+  CUtensorMap tmx, tmw;
+  // one plane of rows [t0 - d, t0 + BLOCK_T + d) per box
+  int rc = planes_map(&tmx, p.src[0], p.src_C[0], p.T, p.B, p.src_rs[0], p.src_bs[0], p.src_ps[0], C::BLOCK_K,
+                      BLOCK_T + 2 * p.dil, 1, "gate_t x");
+  if (rc) return rc;
+  // packed W1 [plane][n_total][k_total], row q gate_tile + h gate_tile / 2 + 8 g + e, as (K, e, h, 8-row group, plane)
+  const int half = p.gate_tile / 2;
+  const cuuint64_t K = (cuuint64_t)p.k_total;
+  const cuuint64_t dims[5] = {K, 8, 2, (cuuint64_t)p.n_total / 8, 2};
+  const cuuint64_t strides[4] = {K * 2, (cuuint64_t)half * K * 2, 8 * K * 2, (cuuint64_t)p.n_total * K * 2};
+  const cuuint32_t box[5] = {(cuuint32_t)C::BLOCK_K, 8, 2, 4, 2};
+  rc = encode_tiled(&tmw, p.w, 5, dims, strides, box, "gate_t w");
+  if (rc) return rc;
+  const int units = p.B * ((p.T + BLOCK_T - 1) / BLOCK_T) * (p.n_total / 128);
+  return fd_tc_launch<fd_gate_t_kernel<BLOCK_T, PREC>>(C::SMEM_BYTES, 2 * units, stream, false, 2, tmx, tmw, p);
+}
+
 template <int BLOCK_N, int BLOCK_K, int EPI, int PREC, int NPL>
 int launch_inst(const FdTapGemm& p, cudaStream_t stream) {
   using C = Cfg<BLOCK_N, BLOCK_K, EPI, NPL>;
@@ -872,6 +1152,10 @@ int fd_tapgemm_tc_launch(const FdTapGemm& p, cudaStream_t stream) {
   FD_REQUIRE(bn != 0 && fd_tapgemm_tc_supported(p),
              "tapgemm(tc): no tensor-core instantiation for n_total=%d k_total=%d epi=%d", p.n_total, p.k_total,
              p.epi);
+  if (const int bt = gate_t_block(p)) {
+    if (bt == 200) return p.prec == FD_F16 ? launch_gate_t<200, FD_F16>(p, stream) : launch_gate_t<200, FD_BF16>(p, stream);
+    return p.prec == FD_F16 ? launch_gate_t<240, FD_F16>(p, stream) : launch_gate_t<240, FD_BF16>(p, stream);
+  }
   if (bk == 64) {
     if (bn == 256) return launch_epi<256, 64>(p, stream);
     if (bn == 128) return launch_epi<128, 64>(p, stream);

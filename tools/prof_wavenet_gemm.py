@@ -12,7 +12,9 @@ from L2 (the two CTAs of a cluster pair each fetch half of the W box and multica
 --hoisted also times the sampler's path: the conditioner projection of all layers computed once per call
 (fd_wavenet_cond_proj, L linear tap-GEMMs with K = E; each launch timed) and GEMM1 over the three conv taps only
 (K = 3C) with the projection added in its epilogue, through fd_wavenet_fwd of a WaveNet with L = 4 layers
-(dilations 1, 2, 4, 8).  TFLOP/s are those of the K each launch actually sums."""
+(dilations 1, 2, 4, 8).  With three products that GEMM1 is the transposed GATE (64 W rows x BLOCK_T = 200 time steps
+per tile, one activation tile per channel block for all three taps); its staged / L2 bytes follow that tiling.
+TFLOP/s are those of the K each launch actually sums."""
 import argparse
 import math
 import os
@@ -25,6 +27,7 @@ sys.path.insert(0, ROOT)
 B, T, C, E = 32, 4000, 512, 256
 BLOCK_M, BLOCK_N = 64, 256
 DILATIONS = (1, 2, 4, 8)
+BLOCK_T = 200                  # the transposed GATE's time tile at T = 4000
 
 
 def staged_bytes(k_total, npl):
@@ -35,6 +38,17 @@ def staged_bytes(k_total, npl):
     a = BLOCK_M * k_total * 2 * npl
     w = BLOCK_N * k_total * 2 * npl
     return tiles * (a + w), tiles * (a + w / 2)
+
+
+def staged_bytes_transposed():
+    """-> (bytes written into shared memory, bytes read from L2) per launch of the transposed GATE (K = 3C, three
+    products), averaged over DILATIONS.  Every (time tile, 64-row W tile) stages, per 32-channel block, the activation
+    rows [t0 - d, t0 + BLOCK_T + d) of both planes once and the three taps' 64-row W boxes; the two CTAs of a pair
+    share the time tile and each fetches one activation plane from L2."""
+    tiles = B * math.ceil(T / BLOCK_T) * (2 * C // 64)
+    w = 3 * 64 * C * 2 * 2
+    act = sum((BLOCK_T + 2 * d) * C * 2 * 2 for d in DILATIONS) / len(DILATIONS)
+    return tiles * (act + w), tiles * (act / 2 + w)
 
 
 def gpu_info():
@@ -136,9 +150,14 @@ def run_hoisted(N, torch, single, reps):
     for name, (ms_sum, n), k, how in rows:
         ms = ms_sum / n
         alg = 2.0 * B * T * (2 * C) * k
+        tiling = ""
+        if how == "read" and not single:
+            staged, l2 = staged_bytes_transposed()
+            tiling = (f" | smem staged {staged / 1e9:5.2f} GB/launch ({staged / ms / 1e9:5.2f} TB/s), "
+                      f"L2 read {l2 / 1e9:5.2f} GB ({l2 / ms / 1e9:5.2f} TB/s)")
         print(f"{name:17s} {ms:7.3f} ms/launch over {n} launches | {alg / ms / 1e9:6.1f} TFLOP/s alg (K={k}), "
               f"{products}x issued = {products * alg / ms / 1e9:6.1f} TFLOP/s | fp32 projection {how} "
-              f"{proj_bytes / 1e9:5.2f} GB/launch ({proj_bytes / ms / 1e6:6.1f} GB/s)", flush=True)
+              f"{proj_bytes / 1e9:5.2f} GB/launch ({proj_bytes / ms / 1e6:6.1f} GB/s){tiling}", flush=True)
     ms_sum, n = fwd_prof["res_skip/tc"]
     print(f"{'GEMM2 res_skip':17s} {ms_sum / n:7.3f} ms/launch over {n} launches", flush=True)
     ms_sum, n = proj_prof["linear/tc"]
