@@ -373,9 +373,24 @@ class Generator(nn.Module):
                                    float(sg.noise_std), seed, N.stream_ptr(dev)), "fd_sinegen_fwd")
         return har
 
+    def _check_source_lengths(self, T):
+        """fd_source_conv_fwd writes (S + 2p - k) / s + 1 rows of noise_convs[i](har) and stage i adds them to its
+        T * prod(rates[:i+1]) rows.  With an odd stride s (upsample rates 3 or 5 after stage i) that is one row short,
+        which the reference refuses with a shape error: refuse it too, before anything is launched."""
+        S = T * int(np.prod(self.h.upsample_rates))
+        L = T
+        for i, (u, nc) in enumerate(zip(self.h.upsample_rates, self.noise_convs)):
+            L *= u
+            k, s, p = nc.kernel_size[0], nc.stride[0], nc.padding[0]
+            n = (S + 2 * p - k) // s + 1
+            if n != L:
+                raise ValueError(f"noise_convs[{i}] (kernel {k}, stride {s}, padding {p}) gives {n} rows of the "
+                                 f"{S}-sample excitation for a stage of {L} rows")
+
     @torch.no_grad()
     def forward(self, x, f0, rand_ini=None, sine_noise=None, seed=None):
         """x mel [B,M,T], f0 [B,T] or [B,1,T] -> wav [B,1,T*hop] (models.py:407-438)."""
+        self._check_source_lengths(x.shape[-1])
         N.require_cuda(x, "mel")
         if f0.ndim == 3:
             f0 = f0[:, 0]

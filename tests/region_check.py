@@ -1,7 +1,7 @@
-"""Error reports of the float64 block tests (test_gpu_wavenet_block.py, test_gpu_wavenet_block_bwd.py): plane values in
-float64, and errors per row region of a [B, T, n] tensor or per named part of a weight gradient, since an error
-confined to a few rows or to one tap's columns vanishes in a whole-tensor rel-L2.  "max" is max|err| in units of the
-whole tensor's RMS."""
+"""Error reports of the float64 block and stage tests (test_gpu_wavenet_block.py, test_gpu_wavenet_block_bwd.py,
+test_gpu_voc_stages.py): plane values in float64, and errors per row region of a [B, T, n] tensor or per named part of
+a weight gradient, since an error confined to a few rows or to one tap's columns vanishes in a whole-tensor rel-L2.
+"max" is max|err| in units of the whole tensor's RMS."""
 import math
 
 import torch
@@ -19,22 +19,35 @@ def pf64(planes, pc, hi_only=False):
 
 
 class Regions:
-    """Per-row-region error accumulation over item chunks: rows [0, dil), [T-dil, T), the last 128-row tile, the rest."""
+    """Per-row-region error accumulation over item chunks: rows [0, dil), [T-dil, T), the last tile (128 rows unless
+    `tile` says otherwise), the rest; with `phase` = P > 1 also each residue class t mod P (a polyphase phase of an
+    upsample, a fold sub-step of a time-folded conv), named f"{phase_name}{r}".  add() takes row windows [t0, t0 + n)
+    of the items, so a few windows of a long tensor are judged by the same regions."""
 
-    def __init__(self, T, dil, device):
-        t = torch.arange(T, device=device)
-        lo, hi, last = t < dil, t >= T - dil, t >= (T - 1) // 128 * 128
-        self.masks = {"all": torch.ones_like(lo), "lo_edge": lo, "hi_edge": hi, "last_tile": last,
-                      "interior": ~(lo | hi | last)}
-        self.se = {k: 0.0 for k in self.masks}
-        self.sr = {k: 0.0 for k in self.masks}
-        self.mx = {k: 0.0 for k in self.masks}
+    def __init__(self, T, dil, device, tile=128, phase=1, phase_name="r"):
+        self.T, self.dil, self.tile, self.phase, self.phase_name = T, dil, tile, phase, phase_name
+        names = ["all", "lo_edge", "hi_edge", "last_tile", "interior"]
+        if phase > 1:
+            names += [f"{phase_name}{r}" for r in range(phase)]
+        self.se = {k: 0.0 for k in names}
+        self.sr = {k: 0.0 for k in names}
+        self.mx = {k: 0.0 for k in names}
         self.n_all = 0
 
-    def add(self, got, ref):
-        """got / ref [b, T, n] float64"""
+    def _masks(self, t):
+        T, dil = self.T, self.dil
+        lo, hi, last = t < dil, t >= T - dil, t >= (T - 1) // self.tile * self.tile
+        masks = {"all": torch.ones_like(lo), "lo_edge": lo, "hi_edge": hi, "last_tile": last,
+                 "interior": ~(lo | hi | last)}
+        if self.phase > 1:
+            for r in range(self.phase):
+                masks[f"{self.phase_name}{r}"] = t % self.phase == r
+        return masks
+
+    def add(self, got, ref, t0=0):
+        """got / ref [b, n, c] float64: rows [t0, t0 + n) of b items"""
         e = got - ref
-        for k, m in self.masks.items():
+        for k, m in self._masks(torch.arange(t0, t0 + ref.shape[1], device=ref.device)).items():
             if not bool(m.any()):
                 continue
             em, rm = e[:, m], ref[:, m]
@@ -47,7 +60,7 @@ class Regions:
         rtol, mtol = tol
         rms = math.sqrt(self.sr["all"] / max(self.n_all, 1))
         msgs, bad = [], []
-        for k in self.masks:
+        for k in self.se:
             if self.sr[k] == 0.0 and self.se[k] == 0.0:
                 continue
             rel = math.sqrt(self.se[k] / max(self.sr[k], 1e-300))
