@@ -111,7 +111,7 @@ template <int C, int PREC>
 __device__ __forceinline__ void rp_gemm(float* acc, const FdResPairK& p, int units, const unsigned char* ul,
                                         unsigned long long km, bool masked, uint32_t a_base, uint32_t a_kb,
                                         uint32_t a_plane, int tap_rows, int row0, uint32_t w_s, int stage_bytes,
-                                        uint64_t* w_full, uint64_t* w_empty, int& stage, uint32_t& phase, int lane) {
+                                        Ring& ring, int lane) {
   using K = RpCfg<C>;
   using MMA = Wgmma<C, PREC>;
   constexpr int KS = K::BKW / 16;
@@ -124,8 +124,8 @@ __device__ __forceinline__ void rp_gemm(float* acc, const FdResPairK& p, int uni
 #pragma unroll 1
   for (int u0 = 0; u0 < units; u0 += p.group) {
     const int nb = min(p.group, units - u0);
-    mbar_wait(&w_full[stage], phase);
-    const uint32_t w_stage = w_s + stage * stage_bytes;
+    ring.wait_full();
+    const uint32_t w_stage = w_s + ring.stage * stage_bytes;
 #pragma unroll 1
     for (int g = 0; g < nb; ++g, ++ui) {
       const int u = masked ? (int)ul[ui] : ui;      // dense convs: no table look-up on the issue path
@@ -150,21 +150,15 @@ __device__ __forceinline__ void rp_gemm(float* acc, const FdResPairK& p, int uni
         wg_fence();
         const uint64_t adv = (uint64_t)((k * 32) >> 4);   // 16 elements * 2 B along K inside the swizzle row
 #pragma unroll
-        for (int j = 0; j < K::BPW; ++j) {
-          float* d = acc + j * (C / 2);
-          if (!single) {
-            MMA::rs(d, alo[j], dw_hi + adv, 1u);
-            MMA::rs(d, ahi[j], dw_lo + adv, 1u);
-          }
-          MMA::rs(d, ahi[j], dw_hi + adv, 1u);
-        }
+        for (int j = 0; j < K::BPW; ++j)
+          split_mma_rs<MMA>(acc + j * (C / 2), ahi[j], alo[j], dw_hi + adv, dw_lo + adv, single);
       }
     }
     wg_commit();
     wg_wait<0>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(&w_empty[stage]);
-    if (++stage == p.nstages) { stage = 0; phase ^= 1; }
+    if (lane == 0) mbar_arrive(&ring.empty[ring.stage]);
+    ring.next();
   }
 }
 
@@ -213,7 +207,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
   if (warp == FD_TC_PRODUCER_WARP) {
     // =========================================================== weight producer (the pair's weights, once per tile)
     if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      Ring ring{w_full, w_empty, p.nstages};
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         for (int g2 = 0; g2 < 2; ++g2) {
           const CUtensorMap* tm = g2 == 0 ? &tm_w1 : &tm_w2;
@@ -222,15 +216,15 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
           const bool pmasked = (g2 == 0 ? p.masked1 : p.masked2) != 0;
           for (int u0 = 0; u0 < units; u0 += p.group) {
             const int nb = min(p.group, units - u0);
-            mbar_wait(&w_empty[stage], phase ^ 1);
-            mbar_expect_tx(&w_full[stage], nb * K::UNIT_BYTES);
-            uint8_t* slot = w_s + stage * STAGE_BYTES_RT;
+            ring.wait_empty();
+            mbar_expect_tx(ring.full_bar(), nb * K::UNIT_BYTES);
+            uint8_t* slot = w_s + ring.stage * STAGE_BYTES_RT;
             for (int g = 0; g < nb; ++g) {
               const int u = pmasked ? (int)ul[u0 + g] : u0 + g;
               const int tap = u / K::UNITS_PER_TAP, kw = u % K::UNITS_PER_TAP;
-              tma_load_3d(slot + g * K::UNIT_BYTES, tm, &w_full[stage], tap * C + kw * K::BKW, 0, 0);
+              tma_load_3d(slot + g * K::UNIT_BYTES, tm, ring.full_bar(), tap * C + kw * K::BKW, 0, 0);
             }
-            if (++stage == p.nstages) { stage = 0; phase ^= 1; }
+            ring.next();
           }
         }
       }
@@ -267,7 +261,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
   const float s2_neg = p.s2 * p.in_slope_inv;
   const float out_c = p.inv_s2 * p.planes_scale, out_cs = out_c * p.out_slope;
   float acc[NACC];
-  int stage = 0; uint32_t phase = 0;
+  Ring ring{w_full, w_empty, p.nstages};
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
     const int b = tile / tiles_t, t0 = (tile % tiles_t) * p.r_out;
@@ -277,7 +271,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
     mbar_wait(in_full, it & 1);
     rp_gemm<C, PREC>(acc, p, p.n1, p.ul1, p.km1, p.masked1 != 0, in_u, in_kb, in_plane, p.d1, blk0 * 64 + 16 * wq,
-                     w_u, STAGE_BYTES_RT, w_full, w_empty, stage, phase, lane);
+                     w_u, STAGE_BYTES_RT, ring, lane);
     wg_fence_operand(acc);
 
     // ---- epilogue 1: bias, LeakyReLU, zero outside [0,T), split planes -> mid tile (c2's A operand).  The mid tile is
@@ -335,7 +329,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
 
     // ---- GEMM2: output rows r, mid rows r + tap
     rp_gemm<C, PREC>(acc, p, p.n2, p.ul2, p.km2, p.masked2 != 0, mid_u, K::MID_KB_BYTES, K::MID_PLANE_BYTES, 1,
-                     blk0 * 64 + 16 * wq, w_u, STAGE_BYTES_RT, w_full, w_empty, stage, phase, lane);
+                     blk0 * 64 + 16 * wq, w_u, STAGE_BYTES_RT, ring, lane);
     wg_fence_operand(acc);
     consumer_sync();                                 // every warpgroup is done reading the mid tile
 

@@ -32,12 +32,6 @@ namespace {
 
 constexpr int BLOCK_M = 128;   // rows of a cooperative tile; a ping-pong tile is one warpgroup's 64
 
-// ring stages of `stage_bytes` that fit next to the fixed parts of shared memory (bias vectors, barriers, scratch)
-constexpr int ring_stages(int stage_bytes, int bias_floats) {
-  return fd_tc_ring_stages(1024 /*align slack*/ + bias_floats * 4 + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES,
-                           stage_bytes);
-}
-
 // NPL = operand planes staged per k-block: 2 (hi + lo, three products) or 1 (hi only, one product: 11-bit (f16) /
 // 8-bit (bf16) operand mantissas, the arithmetic of a plain half-precision tensor-core GEMM with fp32 accumulation).
 template <int BLOCK_N, int BLOCK_K, int EPI, int NPL>
@@ -60,9 +54,8 @@ struct Cfg {
   static constexpr uint32_t SBO = 8 * SWIZZLE_BYTES;
   static constexpr int BIAS_FLOATS = (EPI == FD_EPI_GATE ? 3 : 1) * BLOCK_N;   // one copy of the bias vectors
   static constexpr int BIAS_TOTAL = (PP ? 2 : 1) * BIAS_FLOATS;               // ping-pong: one copy per warpgroup
-  static constexpr int NUM_STAGES = ring_stages(STAGE_BYTES, BIAS_TOTAL);
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + NUM_STAGES * STAGE_BYTES + BIAS_TOTAL * 4 +
-                                    2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
+  static constexpr int NUM_STAGES = fd_tc_frame_stages(STAGE_BYTES, BIAS_TOTAL);
+  static constexpr int SMEM_BYTES = fd_tc_frame_bytes(NUM_STAGES, STAGE_BYTES, BIAS_TOTAL);
   static_assert(NUM_STAGES >= 2, "pipeline needs at least two stages");
   static_assert(SMEM_BYTES <= FD_TC_SMEM_BUDGET, "shared memory");
 };
@@ -461,12 +454,8 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   static_assert(!C::PP, "GATE / RES_SKIP run the ping-pong schedule");
   using MMA = Wgmma<BLOCK_N, PREC>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* stage_base = smem;
-  float* bias_s = reinterpret_cast<float*>(smem + C::NUM_STAGES * C::STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + C::BIAS_TOTAL);
-  uint64_t* empty_bar = full_bar + C::NUM_STAGES;
-  float* scratch_s = reinterpret_cast<float*>(empty_bar + C::NUM_STAGES);   // 16-byte aligned (all preceding sizes are)
+  const TcFrame f = tc_frame(smem_raw, C::NUM_STAGES, C::STAGE_BYTES, C::BIAS_TOTAL);
+  Ring ring{f.full, f.empty, C::NUM_STAGES};
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
@@ -478,22 +467,12 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   int total_k_blocks = 0;
   for (int sI = 0; sI < p.num_seg; ++sI) total_k_blocks += p.seg[sI].k_len / BLOCK_K;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], FD_TC_CONSUMER_THREADS / 32); }
-    fence_barrier_init();
-  }
-  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-    prefetch_tmap(&tm_src0);
-    prefetch_tmap(&tm_src1);
-    prefetch_tmap(&tm_w);
-  }
-  __syncthreads();
+  tc_prologue<false>(f, C::NUM_STAGES, FD_TC_CONSUMER_THREADS / 32, &tm_src0, &tm_src1, &tm_w);
 
   if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
     producer_regs();
     if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_tile = tile / num_n_tiles;
         // rotate the column tile with the row tile: with a grid that is a multiple of num_n_tiles every CTA would
@@ -501,23 +480,22 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
         const int n_tile = (tile % num_n_tiles + m_tile) % num_n_tiles;
         const int b = m_tile / tiles_t, t0 = (m_tile % tiles_t) * BLOCK_M;
         const int n0 = n_tile * BLOCK_N;
-        int s = 0, k0 = 0, koff = 0;                 // flattened (segment, k offset) iterator
+        SegCursor sc;
         for (int kb = 0; kb < total_k_blocks; kb += C::GROUP) {
           const int nb = min(C::GROUP, total_k_blocks - kb);
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* st = stage_base + stage * C::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], nb * C::TX_BYTES);
+          ring.wait_empty();
+          uint8_t* st = f.ring + ring.stage * C::STAGE_BYTES;
+          mbar_expect_tx(ring.full_bar(), nb * C::TX_BYTES);
           for (int g = 0; g < nb; ++g) {
-            const FdSeg sg = p.seg[s];
+            const FdSeg sg = p.seg[sc.s];
             const CUtensorMap* tm = sg.src == 0 ? &tm_src0 : &tm_src1;
             uint8_t* sub = st + g * C::SUB_BYTES;
-            tma_load_4d(sub, tm, &full_bar[stage], sg.c_off + k0, t0 + sg.shift, b, 0);          // hi + lo planes
-            const int kw = koff + k0 + p.w_kshift;
-            tma_load_3d(sub + NPL * C::A_BYTES, &tm_w, &full_bar[stage], kw, n0, 0);               // hi + lo planes
-            k0 += BLOCK_K;
-            if (k0 >= sg.k_len) { koff += sg.k_len; k0 = 0; ++s; }
+            tma_load_4d(sub, tm, ring.full_bar(), sg.c_off + sc.k0, t0 + sg.shift, b, 0);          // hi + lo planes
+            const int kw = sc.koff + sc.k0 + p.w_kshift;
+            tma_load_3d(sub + NPL * C::A_BYTES, &tm_w, ring.full_bar(), kw, n0, 0);                 // hi + lo planes
+            sc.next(BLOCK_K, sg.k_len);
           }
-          if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
+          ring.next();
         }
       }
     }
@@ -528,9 +506,9 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   consumer_regs();
   const int wg = warp / 4;                                   // rows [64 wg, 64 wg + 64) of the tile
   const int wq = warp % 4;                                   // 16-row slice of the warpgroup's 64 rows
-  const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
+  const uint32_t my_scratch = smem_u32(f.scratch) + warp * FD_TC_SCRATCH_WARP_BYTES;
+  float* bias_s = f.bias;
   float acc[BLOCK_N / 2];
-  int stage = 0; uint32_t phase = 0;
   long long staged_key = -1;                                 // which bias vectors shared memory holds
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m_tile = tile / num_n_tiles;
@@ -547,46 +525,18 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
       asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory");
     }
 
-    // ---- mainloop: one wgmma group per ring stage, one group kept in flight; a stage is released once the group
-    //      that read it has completed
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-    int prev_stage = -1;
-    for (int kb = 0; kb < total_k_blocks; kb += C::GROUP) {
-      const int nb = min(C::GROUP, total_k_blocks - kb);
-      mbar_wait(&full_bar[stage], phase);
-      wg_fence_operand(acc);
-      wg_fence();
+    // ---- mainloop: 16 elements * 2 B along K inside the swizzle row per k16 step
+    ring_mainloop(acc, ring, total_k_blocks, C::GROUP, lane, [&](int stage, int nb) {
       for (int g = 0; g < nb; ++g) {
-        const uint32_t st = smem_u32(stage_base + stage * C::STAGE_BYTES + g * C::SUB_BYTES);
+        const uint32_t st = smem_u32(f.ring + stage * C::STAGE_BYTES + g * C::SUB_BYTES);
         const uint32_t wg_a = wg * 64 * C::SWIZZLE_BYTES;     // the warpgroup's 64 rows of a plane
         const uint64_t a_hi = make_smem_desc(st + wg_a, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t a_lo = make_smem_desc(st + C::A_BYTES + wg_a, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t w_hi = make_smem_desc(st + NPL * C::A_BYTES, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t w_lo = make_smem_desc(st + NPL * C::A_BYTES + C::W_BYTES, 16, C::SBO, C::SWIZZLE_MODE);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t adv = (uint64_t)((k * 32) >> 4);   // 16 elements * 2 B along K inside the swizzle row
-          if (NPL == 2) {
-            // small terms first, the dominant hi*hi product last
-            MMA::template ss<0, 0>(acc, a_lo + adv, w_hi + adv, 1u);
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_lo + adv, 1u);
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_hi + adv, 1u);
-          } else {
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_hi + adv, 1u);
-          }
-        }
+        split_mma<MMA, NPL, BLOCK_K / 16, 32>(acc, a_hi, a_lo, w_hi, w_lo);
       }
-      wg_commit();
-      wg_wait<1>();
-      wg_fence_operand(acc);
-      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      prev_stage = stage;
-      if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
-    }
-    wg_wait<0>();
-    wg_fence_operand(acc);
-    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    });
 
     tile_epilogue<BLOCK_N, EPI, PREC>(p, acc, b, n_tile, t0 + wg * 64 + wq * 16, bias_s, my_scratch, lane);
   }
@@ -595,11 +545,8 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
 // ------------------------------------------------------------------ ping-pong schedule (GATE, RES_SKIP)
 // Work unit = (pair of adjacent 64-row tiles, column tile); cluster `pair` takes units pair, pair + num_pairs, ...
 // and its two warpgroups take them in turn (warpgroup 0 the 1st, 3rd, ..., warpgroup 1 the 2nd, 4th, ...).  CTA
-// `rank` of the pair computes row tile 2 m_pair + rank.  The producer fills the ring unit by unit in that order, so the
-// stages of a warpgroup's unit are the total_k_blocks ring positions after the previous unit's.  The mainloops run in
-// turn: a warpgroup waits for its turn (named barrier 1 + wg), and passes it (named barrier 2 - wg) once it has
-// issued the last wgmma group of its tile; its epilogue then overlaps the other warpgroup's mainloop.  The turn also
-// keeps a warpgroup from waiting on a full barrier more than one phase ahead of the ring.
+// `rank` of the pair computes row tile 2 m_pair + rank.  The producer fills the ring unit by unit in that order, and
+// the warpgroups take their turns at the tensor cores (PingPong).
 template <int BLOCK_N, int BLOCK_K, int EPI, int PREC, int NPL>
 __global__ void __launch_bounds__(FD_TC_THREADS, 1)
 fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_constant__ CUtensorMap tm_src1,
@@ -608,12 +555,7 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   static_assert(C::PP && C::GROUP == 1, "ping-pong schedule: GATE / RES_SKIP, one k-block per stage");
   using MMA = Wgmma<BLOCK_N, PREC>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* stage_base = smem;
-  float* bias_s = reinterpret_cast<float*>(smem + C::NUM_STAGES * C::STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + C::BIAS_TOTAL);
-  uint64_t* empty_bar = full_bar + C::NUM_STAGES;
-  float* scratch_s = reinterpret_cast<float*>(empty_bar + C::NUM_STAGES);   // 16-byte aligned (all preceding sizes are)
+  const TcFrame f = tc_frame(smem_raw, C::NUM_STAGES, C::STAGE_BYTES, C::BIAS_TOTAL);
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
@@ -627,23 +569,14 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
   int total_k_blocks = 0;
   for (int sI = 0; sI < p.num_seg; ++sI) total_k_blocks += p.seg[sI].k_len / BLOCK_K;
 
-  if (threadIdx.x == 0) {
-    // a stage is refilled (in both CTAs: W arrives by multicast) once the consuming warpgroup of both CTAs is done
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * 4); }
-    fence_barrier_init();
-  }
-  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-    prefetch_tmap(&tm_src0);
-    prefetch_tmap(&tm_src1);
-    prefetch_tmap(&tm_w);
-  }
-  cluster_sync();   // both CTAs' barriers are initialised before either multicasts or arrives into the other
+  // a stage is refilled (in both CTAs: W arrives by multicast) once the consuming warpgroup of both CTAs is done
+  tc_prologue<true>(f, C::NUM_STAGES, 2 * 4, &tm_src0, &tm_src1, &tm_w);
 
   if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
     producer_regs();
     if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      Ring ring{f.full, f.empty, C::NUM_STAGES};
       for (int u = pair; u < num_units; u += num_pairs) {
         const int m_pair = u / num_n_tiles;
         const int n_tile = (u % num_n_tiles + m_pair) % num_n_tiles;     // rotated as in the cooperative schedule
@@ -652,21 +585,20 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
         const int m_tile = min(2 * m_pair + rank, num_m_tiles - 1);
         const int b = m_tile / tiles_t, t0 = (m_tile % tiles_t) * 64;
         const int n0 = n_tile * BLOCK_N;
-        int s = 0, k0 = 0, koff = 0;                 // flattened (segment, k offset) iterator
+        SegCursor sc;
 #pragma unroll 1                                     // (unrolled, it spills out of the producer's 40 registers)
         for (int kb = 0; kb < total_k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* st = stage_base + stage * C::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], C::TX_BYTES);   // own A box + both halves of W
-          const FdSeg sg = p.seg[s];
-          tma_load_4d(st, sg.src == 0 ? &tm_src0 : &tm_src1, &full_bar[stage], sg.c_off + k0, t0 + sg.shift, b, 0);
+          ring.wait_empty();
+          uint8_t* st = f.ring + ring.stage * C::STAGE_BYTES;
+          mbar_expect_tx(ring.full_bar(), C::TX_BYTES);   // own A box + both halves of W
+          const FdSeg sg = p.seg[sc.s];
+          tma_load_4d(st, sg.src == 0 ? &tm_src0 : &tm_src1, ring.full_bar(), sg.c_off + sc.k0, t0 + sg.shift, b, 0);
           // this CTA's half of the W box -- its plane (three products) or its BLOCK_N / 2 rows (one) -- into both CTAs
-          tma_load_3d_multicast(st + NPL * C::A_BYTES + rank * (NPL * C::W_BYTES / 2), &tm_w, &full_bar[stage],
-                                koff + k0 + p.w_kshift, n0 + (NPL == 1 ? rank * (BLOCK_N / 2) : 0),
+          tma_load_3d_multicast(st + NPL * C::A_BYTES + rank * (NPL * C::W_BYTES / 2), &tm_w, ring.full_bar(),
+                                sc.koff + sc.k0 + p.w_kshift, n0 + (NPL == 1 ? rank * (BLOCK_N / 2) : 0),
                                 NPL == 2 ? rank : 0, 0x3);
-          k0 += BLOCK_K;
-          if (k0 >= sg.k_len) { koff += sg.k_len; k0 = 0; ++s; }
-          if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
+          sc.next(BLOCK_K, sg.k_len);
+          ring.next();
         }
       }
     }
@@ -675,19 +607,10 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
     consumer_regs();
     const int wg = warp / 4;
     const int wq = warp % 4;                                 // 16-row slice of the tile
-    const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
-    float* my_bias = bias_s + wg * C::BIAS_FLOATS;
+    const uint32_t my_scratch = smem_u32(f.scratch) + warp * FD_TC_SCRATCH_WARP_BYTES;
+    float* my_bias = f.bias + wg * C::BIAS_FLOATS;
     float acc[BLOCK_N / 2];
-    int stage = 0; uint32_t phase = 0;
-    auto advance = [&](int n) {                              // n ring positions on
-      stage += n;
-      phase ^= (uint32_t)(stage / C::NUM_STAGES) & 1u;
-      stage %= C::NUM_STAGES;
-    };
-    auto release = [&](int st) {                             // the stage, in both CTAs
-      if (lane == 0) { mbar_arrive_cluster(&empty_bar[st], 0); mbar_arrive_cluster(&empty_bar[st], 1); }
-    };
-    if (wg == 1) advance(total_k_blocks);
+    PingPong turn(f.full, f.empty, C::NUM_STAGES, total_k_blocks, wg);
     long long staged_key = -1;
     for (int u = pair + wg * num_pairs; u < num_units; u += 2 * num_pairs) {
       const int m_pair = u / num_n_tiles;
@@ -705,45 +628,15 @@ fd_tapgemm_pp_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
         wg == 0 ? named_bar_sync<3, 128>() : named_bar_sync<4, 128>();
       }
 
-      if (u != pair) wg == 0 ? named_bar_sync<1, 256>() : named_bar_sync<2, 256>();   // wait for the turn
-      const bool pass = u + num_pairs < num_units;            // the other warpgroup has a next tile
-#pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-      int prev_stage = -1;
-      for (int kb = 0; kb < total_k_blocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        wg_fence_operand(acc);
-        wg_fence();
-        const uint32_t st = smem_u32(stage_base + stage * C::STAGE_BYTES);
+      // `pass`: the other warpgroup has a next tile
+      turn.mainloop(acc, u == pair, u + num_pairs < num_units, lane, [&](int stage) {
+        const uint32_t st = smem_u32(f.ring + stage * C::STAGE_BYTES);
         const uint64_t a_hi = make_smem_desc(st, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t a_lo = make_smem_desc(st + C::A_BYTES, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t w_hi = make_smem_desc(st + NPL * C::A_BYTES, 16, C::SBO, C::SWIZZLE_MODE);
         const uint64_t w_lo = make_smem_desc(st + NPL * C::A_BYTES + C::W_BYTES, 16, C::SBO, C::SWIZZLE_MODE);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t adv = (uint64_t)((k * 32) >> 4);   // 16 elements * 2 B along K inside the swizzle row
-          if (NPL == 2) {
-            // small terms first, the dominant hi*hi product last
-            MMA::template ss<0, 0>(acc, a_lo + adv, w_hi + adv, 1u);
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_lo + adv, 1u);
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_hi + adv, 1u);
-          } else {
-            MMA::template ss<0, 0>(acc, a_hi + adv, w_hi + adv, 1u);
-          }
-        }
-        wg_commit();
-        if (kb == total_k_blocks - 1 && pass)                                   // pass the turn
-          wg == 0 ? named_bar_arrive<2, 256>() : named_bar_arrive<1, 256>();
-        wg_wait<1>();
-        wg_fence_operand(acc);
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        advance(1);
-      }
-      wg_wait<0>();
-      wg_fence_operand(acc);
-      if (prev_stage >= 0) release(prev_stage);
-      advance(total_k_blocks);                                // past the other warpgroup's tile
+        split_mma<MMA, NPL, BLOCK_K / 16, 32>(acc, a_hi, a_lo, w_hi, w_lo);
+      });
 
       if (valid) tile_epilogue<BLOCK_N, EPI, PREC>(p, acc, b, n_tile, t0 + wq * 16, my_bias, my_scratch, lane);
     }
@@ -778,9 +671,8 @@ struct GateTCfg {
   static constexpr int STAGE_BYTES = W_OFF + 3 * 2 * W_PLANE;
   static constexpr uint32_t SWIZZLE_MODE = swizzle_mode_for(ROW_BYTES);
   static constexpr uint32_t SBO = 8 * ROW_BYTES;
-  static constexpr int NUM_STAGES =
-      fd_tc_ring_stages(1024 /*align slack*/ + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES, STAGE_BYTES);
-  static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
+  static constexpr int NUM_STAGES = fd_tc_frame_stages(STAGE_BYTES, 0);
+  static constexpr int SMEM_BYTES = fd_tc_frame_bytes(NUM_STAGES, STAGE_BYTES, 0);
   static_assert(ACT_ROWS <= 256, "one TMA box per plane");
   static_assert(ACT_PLANE % 512 == 0 && STAGE_BYTES % 1024 == 0, "planes start on 64 B swizzle atoms");
   static_assert(NUM_STAGES >= 3, "ring depth");
@@ -867,11 +759,7 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   using C = GateTCfg<BLOCK_T>;
   using MMA = Wgmma<BLOCK_T, PREC>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* stage_base = smem;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::NUM_STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::NUM_STAGES;
-  float* scratch_s = reinterpret_cast<float*>(empty_bar + C::NUM_STAGES);
+  const TcFrame f = tc_frame(smem_raw, C::NUM_STAGES, C::STAGE_BYTES, 0);
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
@@ -884,15 +772,7 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
   const int num_units = p.B * tiles_t * num_wp;
   const int k_blocks = p.C / C::BLOCK_K;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * 4); }
-    fence_barrier_init();
-  }
-  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-    prefetch_tmap(&tm_x);
-    prefetch_tmap(&tm_w);
-  }
-  cluster_sync();
+  tc_prologue<true>(f, C::NUM_STAGES, 2 * 4, &tm_x, &tm_w);
 
   if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
@@ -901,7 +781,7 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
       // both activation planes (one from each CTA of the pair) + this CTA's three W boxes
       const uint32_t tx = 2u * (uint32_t)(BLOCK_T + 2 * d) * C::ROW_BYTES + 3 * 2 * C::W_PLANE;
       const int half = p.gate_tile / 2;
-      int stage = 0; uint32_t phase = 0;
+      Ring ring{f.full, f.empty, C::NUM_STAGES};
       for (int u = pair; u < num_units; u += num_pairs) {
         const int tt = u / num_wp, wt = 2 * (u % num_wp) + rank;
         const int b = tt / tiles_t, t0 = (tt % tiles_t) * BLOCK_T;
@@ -909,16 +789,16 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         const int g0 = ((ch / half) * p.gate_tile + ch % half) / 8;     // its first 8-row group of gate rows
 #pragma unroll 1
         for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* st = stage_base + stage * C::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], tx);
-          tma_load_4d_multicast(st + rank * C::ACT_PLANE, &tm_x, &full_bar[stage], kb * C::BLOCK_K, t0 - d, b, rank,
+          ring.wait_empty();
+          uint8_t* st = f.ring + ring.stage * C::STAGE_BYTES;
+          mbar_expect_tx(ring.full_bar(), tx);
+          tma_load_4d_multicast(st + rank * C::ACT_PLANE, &tm_x, ring.full_bar(), kb * C::BLOCK_K, t0 - d, b, rank,
                                 0x3);
 #pragma unroll 1
           for (int j = 0; j < 3; ++j)
-            tma_load_5d(st + C::W_OFF + j * 2 * C::W_PLANE, &tm_w, &full_bar[stage], j * p.C + kb * C::BLOCK_K, 0, 0,
+            tma_load_5d(st + C::W_OFF + j * 2 * C::W_PLANE, &tm_w, ring.full_bar(), j * p.C + kb * C::BLOCK_K, 0, 0,
                         g0, 0);
-          if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
+          ring.next();
         }
       }
     }
@@ -927,32 +807,15 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     consumer_regs();
     const int wg = warp / 4;
     const int wq = warp % 4;
-    const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
+    const uint32_t my_scratch = smem_u32(f.scratch) + warp * FD_TC_SCRATCH_WARP_BYTES;
     float acc[BLOCK_T / 2];
-    int stage = 0; uint32_t phase = 0;
-    auto advance = [&](int n) {
-      stage += n;
-      phase ^= (uint32_t)(stage / C::NUM_STAGES) & 1u;
-      stage %= C::NUM_STAGES;
-    };
-    auto release = [&](int st) {
-      if (lane == 0) { mbar_arrive_cluster(&empty_bar[st], 0); mbar_arrive_cluster(&empty_bar[st], 1); }
-    };
-    if (wg == 1) advance(k_blocks);
+    PingPong turn(f.full, f.empty, C::NUM_STAGES, k_blocks, wg);
     for (int u = pair + wg * num_pairs; u < num_units; u += 2 * num_pairs) {
       const int tt = u / num_wp, wt = 2 * (u % num_wp) + rank;
       const int b = tt / tiles_t, t0 = (tt % tiles_t) * BLOCK_T;
 
-      if (u != pair) wg == 0 ? named_bar_sync<1, 256>() : named_bar_sync<2, 256>();   // wait for the turn
-      const bool pass = u + num_pairs < num_units;
-#pragma unroll
-      for (int i = 0; i < BLOCK_T / 2; ++i) acc[i] = 0.f;
-      int prev_stage = -1;
-      for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        wg_fence_operand(acc);
-        wg_fence();
-        const uint32_t st = smem_u32(stage_base + stage * C::STAGE_BYTES);
+      turn.mainloop(acc, u == pair, u + num_pairs < num_units, lane, [&](int stage) {
+        const uint32_t st = smem_u32(f.ring + stage * C::STAGE_BYTES);
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
           const uint32_t xa = st + (uint32_t)(j * d * C::ROW_BYTES);       // tap j: activation rows t0 - d + j d ...
@@ -961,27 +824,9 @@ fd_gate_t_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
           const uint32_t wa = st + C::W_OFF + j * 2 * C::W_PLANE;
           const uint64_t w_hi = make_smem_desc(wa, 16, C::SBO, C::SWIZZLE_MODE);
           const uint64_t w_lo = make_smem_desc(wa + C::W_PLANE, 16, C::SBO, C::SWIZZLE_MODE);
-#pragma unroll
-          for (int k = 0; k < C::BLOCK_K / 16; ++k) {
-            const uint64_t adv = (uint64_t)((k * 32) >> 4);
-            // the products in the order of the other orientation: small terms first, hi*hi last
-            MMA::template ss<0, 0>(acc, w_hi + adv, x_lo + adv, 1u);
-            MMA::template ss<0, 0>(acc, w_lo + adv, x_hi + adv, 1u);
-            MMA::template ss<0, 0>(acc, w_hi + adv, x_hi + adv, 1u);
-          }
+          split_mma<MMA, 2, C::BLOCK_K / 16, 32, /*W_IS_A=*/true>(acc, x_hi, x_lo, w_hi, w_lo);
         }
-        wg_commit();
-        if (kb == k_blocks - 1 && pass) wg == 0 ? named_bar_arrive<2, 256>() : named_bar_arrive<1, 256>();
-        wg_wait<1>();
-        wg_fence_operand(acc);
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        advance(1);
-      }
-      wg_wait<0>();
-      wg_fence_operand(acc);
-      if (prev_stage >= 0) release(prev_stage);
-      advance(k_blocks);
+      });
 
       gate_t_epilogue<BLOCK_T, PREC>(p, acc, b, t0, wt * 32 + wq * 8, my_scratch, lane);
     }
@@ -1101,7 +946,7 @@ void pick_cfg(const FdTapGemm& p, int* bn, int* bk) {
   // has the same 2-deep 64-wide ring at BLOCK_N 256 with three products and 5 stages of 40 KB at BLOCK_K 32.)
   const int npl = p.single ? 1 : 2;
   auto wavenet_bk = [&](int n) {
-    return ring_stages(npl * (64 + n) * 64 * 2, 2 * (p.epi == FD_EPI_GATE ? 3 : 1) * n) < 3 ? 32 : 64;
+    return fd_tc_frame_stages(npl * (64 + n) * 64 * 2, 2 * (p.epi == FD_EPI_GATE ? 3 : 1) * n) < 3 ? 32 : 64;
   };
   if (p.epi == FD_EPI_GATE || p.epi == FD_EPI_MAG) {
     const int n = p.gate_tile;

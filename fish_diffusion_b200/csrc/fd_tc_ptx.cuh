@@ -707,6 +707,188 @@ __device__ __forceinline__ float4 scratch_ld4(uint32_t scratch, int row, int chu
   return lds128(scratch + row * 128 + ((chunk ^ (row & 7)) << 4));
 }
 
+// ------------------------------------------------------------------ pipeline plumbing
+// One k-block of the split-precision product on shared-memory operands: KSTEPS k16 steps, the descriptors moving
+// STEP_BYTES per step.  The three products of a step are issued as activation lo x weight hi, activation hi x weight
+// lo, then hi x hi: small terms first, the dominant hi x hi last; every three-product result depends on this order
+// bit for bit.  NPL == 1 issues hi x hi only.  The operands are given by role; W_IS_A puts the weights on the wgmma
+// A (M) side, and TA / TB are the MN-major flags of operands A and B.
+template <class MMA, int NPL, int KSTEPS, int STEP_BYTES, bool W_IS_A = false, int TA = 0, int TB = 0>
+__device__ __forceinline__ void split_mma(float* acc, uint64_t x_hi, uint64_t x_lo, uint64_t w_hi, uint64_t w_lo) {
+  auto mma = [&](uint64_t x, uint64_t w) {
+    if (W_IS_A) MMA::template ss<TA, TB>(acc, w, x, 1u);
+    else MMA::template ss<TA, TB>(acc, x, w, 1u);
+  };
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) {
+    const uint64_t adv = (uint64_t)((k * STEP_BYTES) >> 4);
+    if (NPL == 2) {
+      mma(x_lo + adv, w_hi + adv);
+      mma(x_hi + adv, w_lo + adv);
+    }
+    mma(x_hi + adv, w_hi + adv);
+  }
+}
+// One k16 step of the same products with the activations in registers (MMA::rs, operand A) and the weights K-major
+// in shared memory; `single` issues hi x hi only.
+template <class MMA>
+__device__ __forceinline__ void split_mma_rs(float* acc, const uint32_t (&x_hi)[4], const uint32_t (&x_lo)[4],
+                                             uint64_t w_hi, uint64_t w_lo, bool single) {
+  if (!single) {
+    MMA::rs(acc, x_lo, w_hi, 1u);
+    MMA::rs(acc, x_hi, w_lo, 1u);
+  }
+  MMA::rs(acc, x_hi, w_hi, 1u);
+}
+
+// Cursor of a full / empty barrier ring of `stages` stages: the stage the next access goes to and the phase parity of
+// its barriers.  The producer waits for a stage to be empty, the consumers for it to be full.  Where `stages` is a
+// compile-time constant it folds into the code as the constant would.
+struct Ring {
+  uint64_t* full;
+  uint64_t* empty;
+  int stages;
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ uint64_t* full_bar() const { return &full[stage]; }
+  __device__ __forceinline__ void wait_full() const { mbar_wait(&full[stage], phase); }
+  __device__ __forceinline__ void wait_empty() const { mbar_wait(&empty[stage], phase ^ 1); }
+  __device__ __forceinline__ void next() {
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  __device__ __forceinline__ void advance(int n) {   // n ring positions on
+    stage += n;
+    phase ^= (uint32_t)(stage / stages) & 1u;
+    stage %= stages;
+  }
+};
+
+// The mainloop of a consumer warpgroup of the cooperative kernels over `k_blocks` k-blocks, `group` of them per ring
+// stage: one wgmma group per stage, issued by issue(stage, k-blocks in the stage), and one group kept in flight; lane
+// 0 of each warp releases a stage once the group that read it has completed.  The accumulators start at zero.
+template <int R, class Issue>
+__device__ __forceinline__ void ring_mainloop(float (&acc)[R], Ring& ring, int k_blocks, int group, int lane,
+                                              Issue&& issue) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = 0.f;
+  int prev_stage = -1;
+  for (int kb = 0; kb < k_blocks; kb += group) {
+    ring.wait_full();
+    wg_fence_operand(acc);
+    wg_fence();
+    issue(ring.stage, min(group, k_blocks - kb));
+    wg_commit();
+    wg_wait<1>();
+    wg_fence_operand(acc);
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(&ring.empty[prev_stage]);
+    prev_stage = ring.stage;
+    ring.next();
+  }
+  wg_wait<0>();
+  wg_fence_operand(acc);
+  if (prev_stage >= 0 && lane == 0) mbar_arrive(&ring.empty[prev_stage]);
+}
+
+// The ping-pong turn of the two consumer warpgroups of a CTA in a 2x1x1 cluster (fd_tapgemm_tc.cu).  The producer
+// fills one ring for both warpgroups, unit by unit, each unit `k_blocks` stages; warpgroup 0 takes the 1st, 3rd, ...
+// unit, warpgroup 1 the 2nd, 4th, ...  The mainloops run in turn: a warpgroup waits for its turn (named barrier
+// 1 + wg) and passes it (named barrier 2 - wg) once it has committed the last wgmma group of its unit, so that its
+// epilogue overlaps the other warpgroup's mainloop.  The turn also keeps a warpgroup from waiting on a full barrier
+// more than one phase ahead of the ring.  A stage is refilled in both CTAs (the weights arrive by multicast), so it is
+// released into both.
+struct PingPong {
+  Ring ring;
+  int k_blocks;
+  int wg;
+  __device__ __forceinline__ PingPong(uint64_t* full, uint64_t* empty, int stages, int k_blocks_, int wg_)
+      : ring{full, empty, stages}, k_blocks(k_blocks_), wg(wg_) {
+    if (wg == 1) ring.advance(k_blocks);
+  }
+  // One unit's mainloop, the accumulators from zero; `first`: the warpgroup's first unit (no turn to wait for),
+  // `pass`: the other warpgroup has a next unit.  issue(stage) issues the wgmma group of one stage; one group is kept
+  // in flight, as in ring_mainloop.  The ring steps by advance(1): with next() the compiler unrolls this loop and
+  // triples the code of a three-product stage.
+  template <int R, class Issue>
+  __device__ __forceinline__ void mainloop(float (&acc)[R], bool first, bool pass, int lane, Issue&& issue) {
+    auto release = [&](int st) {
+      if (lane == 0) { mbar_arrive_cluster(&ring.empty[st], 0); mbar_arrive_cluster(&ring.empty[st], 1); }
+    };
+    if (!first) wg == 0 ? named_bar_sync<1, 256>() : named_bar_sync<2, 256>();       // wait for the turn
+#pragma unroll
+    for (int i = 0; i < R; ++i) acc[i] = 0.f;
+    int prev_stage = -1;
+    for (int kb = 0; kb < k_blocks; ++kb) {
+      ring.wait_full();
+      wg_fence_operand(acc);
+      wg_fence();
+      issue(ring.stage);
+      wg_commit();
+      if (kb == k_blocks - 1 && pass) wg == 0 ? named_bar_arrive<2, 256>() : named_bar_arrive<1, 256>();   // pass it
+      wg_wait<1>();
+      wg_fence_operand(acc);
+      if (prev_stage >= 0) release(prev_stage);
+      prev_stage = ring.stage;
+      ring.advance(1);
+    }
+    wg_wait<0>();
+    wg_fence_operand(acc);
+    if (prev_stage >= 0) release(prev_stage);
+    ring.advance(k_blocks);   // past the other warpgroup's unit
+  }
+};
+
+// Shared memory of a warp-specialised tensor-core kernel, from the 1024-byte aligned base: the ring of `stages` stages
+// of `stage_bytes`, `bias_floats` floats of bias vectors, the full and empty barriers, the consumer warps' scratch
+// (16-byte aligned: every preceding size is).
+constexpr int fd_tc_frame_bytes(int stages, int stage_bytes, int bias_floats) {
+  return 1024 /*align slack*/ + stages * stage_bytes + bias_floats * 4 + 2 * stages * 8 + FD_TC_SCRATCH_BYTES;
+}
+// ring stages of `stage_bytes` that fit next to the rest of that frame
+constexpr int fd_tc_frame_stages(int stage_bytes, int bias_floats) {
+  return fd_tc_ring_stages(fd_tc_frame_bytes(FD_TC_MAX_STAGES, 0, bias_floats), stage_bytes);
+}
+struct TcFrame {
+  uint8_t* ring;
+  float* bias;
+  uint64_t* full;
+  uint64_t* empty;
+  float* scratch;
+};
+__device__ __forceinline__ TcFrame tc_frame(uint8_t* smem_raw, int stages, int stage_bytes, int bias_floats) {
+  TcFrame f;
+  f.ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  f.bias = reinterpret_cast<float*>(f.ring + stages * stage_bytes);
+  f.full = reinterpret_cast<uint64_t*>(f.bias + bias_floats);
+  f.empty = f.full + stages;
+  f.scratch = reinterpret_cast<float*>(f.empty + stages);
+  return f;
+}
+// The prologue: thread 0 initialises the ring's barriers (a full barrier completes on the producer's arrival and its
+// transaction bytes, an empty barrier on `empty_arrivals` consumer warps), the producer thread prefetches the tensor
+// maps, then the CTA -- or with CLUSTER the whole cluster, so that no CTA multicasts or arrives into a peer whose
+// barriers are not initialised -- synchronises.
+template <bool CLUSTER, class... Maps>
+__device__ __forceinline__ void tc_prologue(const TcFrame& f, int stages, uint32_t empty_arrivals,
+                                            const Maps*... maps) {
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < stages; ++i) { mbar_init(&f.full[i], 1); mbar_init(&f.empty[i], empty_arrivals); }
+    fence_barrier_init();
+  }
+  if (threadIdx.x / 32 == FD_TC_PRODUCER_WARP && threadIdx.x % 32 == 0) (prefetch_tmap(maps), ...);
+  if (CLUSTER) cluster_sync();
+  else __syncthreads();
+}
+
+// The producer's walk over the K segments of a tap-GEMM: segment s, k offset k0 inside it, and koff, the packed weight
+// column of the segment's first k.
+struct SegCursor {
+  int s = 0, k0 = 0, koff = 0;
+  __device__ __forceinline__ void next(int block_k, int k_len) {   // one k-block on; k_len of segment s
+    k0 += block_k;
+    if (k0 >= k_len) { koff += k_len; k0 = 0; ++s; }
+  }
+};
+
 // ------------------------------------------------------------------ host side: tensor-map encoder entry point
 typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,

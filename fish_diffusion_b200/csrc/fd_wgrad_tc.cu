@@ -32,10 +32,8 @@ struct WgCfg {
   static constexpr int A_BYTES = A_BOXES * NPL * WG_BOX_BYTES;
   static constexpr int W_BYTES = W_BOXES * NPL * WG_BOX_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
-  // next to the align slack, the barriers and the scratch
-  static constexpr int NUM_STAGES =
-      fd_tc_ring_stages(1024 + 2 * FD_TC_MAX_STAGES * 8 + FD_TC_SCRATCH_BYTES, STAGE_BYTES);
-  static constexpr int SMEM_BYTES = 1024 + NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + FD_TC_SCRATCH_BYTES;
+  static constexpr int NUM_STAGES = fd_tc_frame_stages(STAGE_BYTES, 0);
+  static constexpr int SMEM_BYTES = fd_tc_frame_bytes(NUM_STAGES, STAGE_BYTES, 0);
   static_assert(NUM_STAGES >= 2, "pipeline needs at least two stages");
 };
 
@@ -47,11 +45,8 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   using C = WgCfg<BLOCK_N, NPL>;
   using MMA = Wgmma<BLOCK_N, PREC>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* stage_base = smem;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::NUM_STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::NUM_STAGES;
-  float* scratch_s = reinterpret_cast<float*>(empty_bar + C::NUM_STAGES);
+  const TcFrame f = tc_frame(smem_raw, C::NUM_STAGES, C::STAGE_BYTES, 0);
+  Ring ring{f.full, f.empty, C::NUM_STAGES};
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
@@ -59,20 +54,12 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   const int num_units = p.splits * tiles_per_split;
   const int k_blocks = (p.T + WG_BLOCK_K - 1) / WG_BLOCK_K;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < C::NUM_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], FD_TC_CONSUMER_THREADS / 32); }
-    fence_barrier_init();
-  }
-  if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-    prefetch_tmap(&tm_row0); prefetch_tmap(&tm_row1); prefetch_tmap(&tm_col0); prefetch_tmap(&tm_col1);
-  }
-  __syncthreads();
+  tc_prologue<false>(f, C::NUM_STAGES, FD_TC_CONSUMER_THREADS / 32, &tm_row0, &tm_row1, &tm_col0, &tm_col1);
 
   if (warp >= FD_TC_PRODUCER_WARP) {
     // =========================================================== TMA producer
     producer_regs();
     if (warp == FD_TC_PRODUCER_WARP && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         const int s = unit / tiles_per_split;
         const int tile = unit % tiles_per_split;
@@ -105,17 +92,17 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
         for (int b = s * p.items_per_split; b < b_end; ++b) {
           for (int kb = 0; kb < k_blocks; ++kb) {
             const int t0 = kb * WG_BLOCK_K;
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* st = stage_base + stage * C::STAGE_BYTES;
-            mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+            ring.wait_empty();
+            uint8_t* st = f.ring + ring.stage * C::STAGE_BYTES;
+            mbar_expect_tx(ring.full_bar(), C::STAGE_BYTES);
 #pragma unroll
             for (int i = 0; i < C::A_BOXES; ++i)
-              tma_load_4d(st + i * NPL * WG_BOX_BYTES, a_map[i], &full_bar[stage], a_ch[i], t0, b, 0);
+              tma_load_4d(st + i * NPL * WG_BOX_BYTES, a_map[i], ring.full_bar(), a_ch[i], t0, b, 0);
 #pragma unroll
             for (int i = 0; i < C::W_BOXES; ++i)
-              tma_load_4d(st + C::A_BYTES + i * NPL * WG_BOX_BYTES, w_map[i], &full_bar[stage], w_ch[i], t0 + w_sh[i],
+              tma_load_4d(st + C::A_BYTES + i * NPL * WG_BOX_BYTES, w_map[i], ring.full_bar(), w_ch[i], t0 + w_sh[i],
                           b, 0);
-            if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
+            ring.next();
           }
         }
       }
@@ -127,51 +114,25 @@ fd_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_row0, const __grid_con
   consumer_regs();
   const int wg = warp / 4;                           // rows [64 wg, 64 wg + 64) of the tile = A box wg
   const int wq = warp % 4;
-  const uint32_t my_scratch = smem_u32(scratch_s) + warp * FD_TC_SCRATCH_WARP_BYTES;
+  const uint32_t my_scratch = smem_u32(f.scratch) + warp * FD_TC_SCRATCH_WARP_BYTES;
   const int j4 = (lane & 7) * 4, rsub = lane >> 3;
   // MN-major SW128 operands: LBO = distance between 64-channel atoms (the boxes), SBO = 8 time rows of 128 bytes
   constexpr uint32_t LBO = NPL * WG_BOX_BYTES, SBO = 1024;
   float acc[BLOCK_N / 2];
-  int stage = 0; uint32_t phase = 0;
   for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
     const int s = unit / tiles_per_split;
     const int tile = unit % tiles_per_split;
     const int r0 = (tile / p.n_tiles) * WG_BLOCK_M, c0 = (tile % p.n_tiles) * BLOCK_N;
     const int n_items = min(p.B, (s + 1) * p.items_per_split) - s * p.items_per_split;
-    const int total = n_items * k_blocks;
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-    int prev_stage = -1;
-    for (int it = 0; it < total; ++it) {
-      mbar_wait(&full_bar[stage], phase);
-      wg_fence_operand(acc);
-      wg_fence();
-      const uint32_t st = smem_u32(stage_base + stage * C::STAGE_BYTES);
+    ring_mainloop(acc, ring, n_items * k_blocks, 1, lane, [&](int stage, int) {
+      const uint32_t st = smem_u32(f.ring + stage * C::STAGE_BYTES);
       const uint64_t a_hi = make_smem_desc(st + wg * NPL * WG_BOX_BYTES, LBO, SBO, 1);
       const uint64_t a_lo = make_smem_desc(st + wg * NPL * WG_BOX_BYTES + WG_BOX_BYTES, LBO, SBO, 1);
       const uint64_t w_hi = make_smem_desc(st + C::A_BYTES, LBO, SBO, 1);
       const uint64_t w_lo = make_smem_desc(st + C::A_BYTES + WG_BOX_BYTES, LBO, SBO, 1);
-#pragma unroll
-      for (int k = 0; k < WG_BLOCK_K / 16; ++k) {
-        const uint64_t adv = (uint64_t)((k * 16 * 128) >> 4);      // 16 time rows of 128 bytes
-        if (NPL == 2) {
-          MMA::template ss<1, 1>(acc, a_lo + adv, w_hi + adv, 1u);
-          MMA::template ss<1, 1>(acc, a_hi + adv, w_lo + adv, 1u);
-          MMA::template ss<1, 1>(acc, a_hi + adv, w_hi + adv, 1u);
-        } else {
-          MMA::template ss<1, 1>(acc, a_hi + adv, w_hi + adv, 1u);
-        }
-      }
-      wg_commit();
-      wg_wait<1>();
-      wg_fence_operand(acc);
-      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      prev_stage = stage;
-      if (++stage == C::NUM_STAGES) { stage = 0; phase ^= 1; }
-    }
-    wg_wait<0>();
-    wg_fence_operand(acc);
-    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      // k16 steps of 16 time rows of 128 bytes
+      split_mma<MMA, NPL, WG_BLOCK_K / 16, 16 * 128, false, 1, 1>(acc, a_hi, a_lo, w_hi, w_lo);
+    });
 
     // ---- epilogue: 32-column chunks through the warp scratch; 8 lanes cover one 128-byte row segment
     float* const out = p.part + (size_t)s * p.R * p.Cc;
