@@ -201,10 +201,6 @@ __device__ __forceinline__ void fd_dgate(float dz, float g, float f, float& dg, 
 // ------------------------------------------------------------------------------------------------
 // vector helpers: V consecutive channels (V = 4 or 8)
 // ------------------------------------------------------------------------------------------------
-template <int V> struct FdVec16;   // V x uint16
-template <> struct FdVec16<4> { uint2 v; };
-template <> struct FdVec16<8> { uint4 v; };
-
 // two neighbouring channels at once: ONE packed, saturating conversion per plane word (F2FP.SATFINITE.*.PACK_AB)
 // instead of clamp + convert + pack per element.  a -> low half-word, b -> high half-word.  Bit-identical to fd_split
 // for |v| <= 65504 (f16) / all finite v (bf16).
@@ -238,22 +234,18 @@ __device__ __forceinline__ void fd_store_planes(uint16_t* planes, size_t plane_e
 template <int V>
 __device__ __forceinline__ void fd_load_planes(const uint16_t* planes, size_t plane_elems, size_t off,
                                                float (&y)[V], int prec) {
-  uint16_t hi[8], lo[8];
+  uint32_t hi[4], lo[4];
   if (V == 4) {
-    uint2 a = *reinterpret_cast<const uint2*>(planes + off);
-    uint2 b = *reinterpret_cast<const uint2*>(planes + plane_elems + off);
-    hi[0] = a.x & 0xffff; hi[1] = a.x >> 16; hi[2] = a.y & 0xffff; hi[3] = a.y >> 16;
-    lo[0] = b.x & 0xffff; lo[1] = b.x >> 16; lo[2] = b.y & 0xffff; lo[3] = b.y >> 16;
+    const uint2 a = *reinterpret_cast<const uint2*>(planes + off);
+    const uint2 b = *reinterpret_cast<const uint2*>(planes + plane_elems + off);
+    hi[0] = a.x; hi[1] = a.y; lo[0] = b.x; lo[1] = b.y;
   } else {
-    uint4 a = *reinterpret_cast<const uint4*>(planes + off);
-    uint4 b = *reinterpret_cast<const uint4*>(planes + plane_elems + off);
-    hi[0] = a.x & 0xffff; hi[1] = a.x >> 16; hi[2] = a.y & 0xffff; hi[3] = a.y >> 16;
-    hi[4] = a.z & 0xffff; hi[5] = a.z >> 16; hi[6] = a.w & 0xffff; hi[7] = a.w >> 16;
-    lo[0] = b.x & 0xffff; lo[1] = b.x >> 16; lo[2] = b.y & 0xffff; lo[3] = b.y >> 16;
-    lo[4] = b.z & 0xffff; lo[5] = b.z >> 16; lo[6] = b.w & 0xffff; lo[7] = b.w >> 16;
+    const uint4 a = *reinterpret_cast<const uint4*>(planes + off);
+    const uint4 b = *reinterpret_cast<const uint4*>(planes + plane_elems + off);
+    hi[0] = a.x; hi[1] = a.y; hi[2] = a.z; hi[3] = a.w; lo[0] = b.x; lo[1] = b.y; lo[2] = b.z; lo[3] = b.w;
   }
 #pragma unroll
-  for (int i = 0; i < V; ++i) y[i] = fd_combine(hi[i], lo[i], prec);
+  for (int i = 0; i < V / 2; ++i) fd_combine2(hi[i], lo[i], prec, y[2 * i], y[2 * i + 1]);
 }
 
 // hi plane only (single-product mode of the SIMT twin)
@@ -265,25 +257,6 @@ __device__ __forceinline__ void fd_load_hi8(const uint16_t* planes, size_t off, 
     y[2 * i] = fd_h2f((uint16_t)(w[i] & 0xffff), prec);
     y[2 * i + 1] = fd_h2f((uint16_t)(w[i] >> 16), prec);
   }
-}
-
-// register-level (un)packing of 8 consecutive channels; used by the split-phase (prefetch / finish) epilogues
-__device__ __forceinline__ void fd_unpack8(const uint4& a, const uint4& b, int prec, float (&y)[8]) {
-  const uint32_t ha[4] = {a.x, a.y, a.z, a.w}, lb[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    y[2 * i] = fd_combine((uint16_t)(ha[i] & 0xffff), (uint16_t)(lb[i] & 0xffff), prec);
-    y[2 * i + 1] = fd_combine((uint16_t)(ha[i] >> 16), (uint16_t)(lb[i] >> 16), prec);
-  }
-}
-__device__ __forceinline__ void fd_pack8(const float (&y)[8], int prec, uint4& a, uint4& b) {
-  uint16_t hi[8], lo[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) fd_split(y[i], prec, hi[i], lo[i]);
-  a.x = hi[0] | ((uint32_t)hi[1] << 16); a.y = hi[2] | ((uint32_t)hi[3] << 16);
-  a.z = hi[4] | ((uint32_t)hi[5] << 16); a.w = hi[6] | ((uint32_t)hi[7] << 16);
-  b.x = lo[0] | ((uint32_t)lo[1] << 16); b.y = lo[2] | ((uint32_t)lo[3] << 16);
-  b.z = lo[4] | ((uint32_t)lo[5] << 16); b.w = lo[6] | ((uint32_t)lo[7] << 16);
 }
 
 template <int V>
@@ -302,106 +275,280 @@ __device__ __forceinline__ void fd_store_f32(float* p, const float (&y)[V]) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Epilogues.  Each handles V consecutive output columns [n0, n0+V) of row (b,t) with raw
-// accumulators acc[].  `bias*` pointers may be shared-memory or global (generic loads).
+// Epilogues: one definition per kind, used by every tap-GEMM kernel (the wgmma kernels' wide and narrow column tiles
+// and the SIMT twin).  A kernel maps its accumulators to a fragment of R rows x V consecutive columns of one item,
+// loads the bias values of those columns its own way and passes them in; PREC is compile-time in the tensor-core
+// kernel (-1: p.prec).
 // ------------------------------------------------------------------------------------------------
-template <int V, int PREC = -1>
-__device__ __forceinline__ void fd_epi_linear(const FdTapGemm& p, int b, int t, int n0,
-                                              const float (&acc)[V], const float* bias_tile /*[n - tile_n0] or null*/,
-                                              int tile_n0) {
-  const int prec = PREC < 0 ? p.prec : PREC;   // compile-time in the tensor-core kernel
-  const size_t row = (size_t)b * p.T + t;
-  const size_t off = row * p.n_total + n0;
-  const size_t plane_elems = (size_t)p.B * p.T * p.n_total;
-  float y[V];
-  const bool masked = p.row_mask != nullptr && p.row_mask[row] != 0;
+// The rows of a fragment: time steps t0, t0 + dt, ..., t0 + (R - 1) dt of one item.  The first nrows lie inside the
+// item and are stored; the loads of the others are clamped to its last step.  I is the type of the element offsets:
+// 32-bit in the tensor-core kernel (its launch checks the output sizes), 64-bit in the SIMT twin.
+template <typename I>
+struct FdRows {
+  I item;   // b * T
+  int t0, dt, nrows;
+  __device__ __forceinline__ I row(const FdTapGemm& p, int r) const { return item + (I)min(t0 + r * dt, p.T - 1); }
+};
+
+// packed column of gate channel c: column tiles of gate_tile hold gate_tile / 2 gates, then their filters
+__device__ __forceinline__ int fd_gate_col(const FdTapGemm& p, int c) {
+  const int half = p.gate_tile / 2;
+  return (c / half) * p.gate_tile + c % half;
+}
+
+// LINEAR: columns [n, n + V) of the fragment's rows, `a` the raw accumulators.  All loads are issued before the
+// first store.
+//   y = (a*acc_scale + bias + (addend + res_f32 + res_scale*res_planes)) * post_scale;  y += out_f32 if out_accum;
+//   rows with row_mask != 0 are zeros;  out_f32 = y,  out_planes = split(act(y * planes_scale)).
+template <int R, int V, int PREC, typename I>
+__device__ __forceinline__ void fd_epi_linear(const FdTapGemm& p, const FdRows<I>& rw, int n, float (&a)[R][V],
+                                              const float (&bias)[V]) {
+  const int prec = PREC < 0 ? p.prec : PREC;
+  const size_t plane = (size_t)p.B * p.T * p.n_total;
+  I off[R];
+  float pre[R][V];
 #pragma unroll
-  for (int i = 0; i < V; ++i) y[i] = acc[i] * p.acc_scale;
-  if (bias_tile != nullptr) {
+  for (int r = 0; r < R; ++r) {
+    off[r] = rw.row(p, r) * (I)p.n_total + (I)n;
 #pragma unroll
-    for (int i = 0; i < V; ++i) y[i] += bias_tile[n0 - tile_n0 + i];
+    for (int i = 0; i < V; ++i) pre[r][i] = 0.f;
   }
   if (p.addend != nullptr) {
-    float a[V]; fd_load_f32<V>(p.addend + off, a);
 #pragma unroll
-    for (int i = 0; i < V; ++i) y[i] += a[i];
+    for (int r = 0; r < R; ++r) {
+      float v[V];
+      fd_load_f32<V>(p.addend + off[r], v);
+#pragma unroll
+      for (int i = 0; i < V; ++i) pre[r][i] += v[i];
+    }
   }
   if (p.res_f32 != nullptr) {
-    float a[V]; fd_load_f32<V>(p.res_f32 + off, a);
 #pragma unroll
-    for (int i = 0; i < V; ++i) y[i] += a[i];
+    for (int r = 0; r < R; ++r) {
+      float v[V];
+      fd_load_f32<V>(p.res_f32 + off[r], v);
+#pragma unroll
+      for (int i = 0; i < V; ++i) pre[r][i] += v[i];
+    }
   }
   if (p.res_planes != nullptr) {
-    float a[V]; fd_load_planes<V>(p.res_planes, plane_elems, off, a, prec);
 #pragma unroll
-    for (int i = 0; i < V; ++i) y[i] += a[i] * p.res_scale;
+    for (int r = 0; r < R; ++r) {
+      float v[V];
+      fd_load_planes<V>(p.res_planes, plane, off[r], v, prec);
+#pragma unroll
+      for (int i = 0; i < V; ++i) pre[r][i] += p.res_scale * v[i];
+    }
+  }
+  uint32_t masked = 0;
+  if (p.row_mask != nullptr) {
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if (p.row_mask[rw.row(p, r)] != 0) masked |= 1u << r;
   }
 #pragma unroll
-  for (int i = 0; i < V; ++i) y[i] *= p.post_scale;
-  if (p.out_f32 != nullptr) {
-    if (p.out_accum) {
-      float a[V]; fd_load_f32<V>(p.out_f32 + off, a);
+  for (int r = 0; r < R; ++r)
 #pragma unroll
-      for (int i = 0; i < V; ++i) y[i] += a[i];
-    }
-    if (masked) {
+    for (int i = 0; i < V; ++i) a[r][i] = (a[r][i] * p.acc_scale + bias[i] + pre[r][i]) * p.post_scale;
+  if (p.out_f32 != nullptr && p.out_accum) {
 #pragma unroll
-      for (int i = 0; i < V; ++i) y[i] = 0.f;
+    for (int r = 0; r < R; ++r) {
+      float v[V];
+      fd_load_f32<V>(p.out_f32 + off[r], v);
+#pragma unroll
+      for (int i = 0; i < V; ++i) a[r][i] += v[i];
     }
-    fd_store_f32<V>(p.out_f32 + off, y);
   }
-  if (p.out_planes != nullptr) {
+  const float slope = p.act == FD_ACT_NONE ? 1.f : p.act == FD_ACT_RELU ? 0.f : p.act_slope;
 #pragma unroll
-    for (int i = 0; i < V; ++i) {
-      float v = y[i] * p.planes_scale;
-      if (p.act == FD_ACT_RELU) v = fmaxf(v, 0.f);
-      else if (p.act == FD_ACT_LRELU) v = v > 0.f ? v : v * p.act_slope;
-      y[i] = masked ? 0.f : v;
+  for (int r = 0; r < R; ++r) {
+    if (r >= rw.nrows) break;
+    if ((masked >> r) & 1u) {
+#pragma unroll
+      for (int i = 0; i < V; ++i) a[r][i] = 0.f;
     }
-    fd_store_planes<V>(p.out_planes, plane_elems, off, y, prec);
+    if (p.out_f32 != nullptr) fd_store_f32<V>(p.out_f32 + off[r], a[r]);
+    if (p.out_planes != nullptr) {
+      float v[V];
+#pragma unroll
+      for (int i = 0; i < V; ++i) v[i] = fd_act(a[r][i] * p.planes_scale, slope);
+      fd_store_planes<V>(p.out_planes, plane, off[r], v, prec);
+    }
   }
 }
 
-// gate epilogue: V gate accumulators + V filter accumulators for residual channels [zc0, zc0+V);
-// *_g point at the bias of the FIRST gate column of this thread's chunk, *_f at the first filter col.
-// n_g / n_f: the packed columns of those two (for the addend).
-template <int V, int PREC = -1>
-__device__ __forceinline__ void fd_epi_gate(const FdTapGemm& p, int b, int t, int zc0, int n_g, int n_f,
-                                            const float (&g)[V], const float (&f)[V],
-                                            const float* full_g, const float* full_f,
-                                            const float* lo_g, const float* lo_f,
-                                            const float* hi_g, const float* hi_f) {
-  const int prec = PREC < 0 ? p.prec : PREC;   // compile-time in the tensor-core kernel
-  float z[V], yg8[V], yf8[V], ag[V], af[V];
-  const bool e_lo = t < p.dil, e_hi = t + p.dil >= p.T;
-  if (p.addend != nullptr) {
-    const size_t arow = ((size_t)b * p.T + t) * p.n_total;
-    fd_load_f32<V>(p.addend + arow + n_g, ag);
-    fd_load_f32<V>(p.addend + arow + n_f, af);
+// RES_SKIP (WaveNet GEMM2): packed columns [0, C) are the residual half, [C, 2C) the skip half; y = a*acc_scale + bias.
+//   residual: x = (x + y) / sqrt(2) on the split planes (into x_out_planes if set); not in the last layer, whose
+//   residual stream is not consumed;
+//   skip: y += skip_f32 except in the first layer; the last layer writes split(y * skip_scale) to skip_planes, the
+//   others y to skip_f32.
+// is_res = n < C, passed in so that a kernel whose column tiles lie in one half can make it a warp-uniform branch.
+template <int R, int V, int PREC, typename I>
+__device__ __forceinline__ void fd_epi_res_skip(const FdTapGemm& p, const FdRows<I>& rw, int n, bool is_res,
+                                                const float (&a)[R][V], const float (&bias)[V]) {
+  const int prec = PREC < 0 ? p.prec : PREC;
+  const size_t plane = (size_t)p.B * p.T * p.C;
+  const I cn = (I)(is_res ? n : n - p.C);
+  I off[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) off[r] = rw.row(p, r) * (I)p.C + cn;
+  if (is_res) {
+    if (p.last_layer) return;
+    float x[R][V];
+#pragma unroll
+    for (int r = 0; r < R; ++r) fd_load_planes<V>(p.x_planes, plane, off[r], x[r], prec);
+    uint16_t* const xo = p.x_out_planes != nullptr ? p.x_out_planes : p.x_planes;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (r >= rw.nrows) break;
+#pragma unroll
+      for (int i = 0; i < V; ++i) x[r][i] = (x[r][i] + (a[r][i] * p.acc_scale + bias[i])) * 0.70710678118654752440f;
+      fd_store_planes<V>(xo, plane, off[r], x[r], prec);
+    }
+  } else {
+    float sk[R][V];
+    if (!p.first_layer) {
+#pragma unroll
+      for (int r = 0; r < R; ++r) fd_load_f32<V>(p.skip_f32 + off[r], sk[r]);
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (r >= rw.nrows) break;
+      float y[V];
+#pragma unroll
+      for (int i = 0; i < V; ++i) {
+        y[i] = a[r][i] * p.acc_scale + bias[i];
+        if (!p.first_layer) y[i] += sk[r][i];
+      }
+      if (p.last_layer) {
+#pragma unroll
+        for (int i = 0; i < V; ++i) y[i] *= p.skip_scale;
+        fd_store_planes<V>(p.skip_planes, plane, off[r], y, prec);
+      } else {
+        fd_store_f32<V>(p.skip_f32 + off[r], y);
+      }
+    }
   }
+}
+
+// GATE (WaveNet GEMM1) at time step t: g and f hold the raw accumulators of V gate columns and of their V filter
+// columns and leave as the pre-activations
+//   y = acc*acc_scale + bias + addend - [t < dil] lo - [t + dil >= T] hi;   z = sigmoid(y_gate) tanh(y_filter).
+// bias, add, lo and hi hold the gate values in [0] and the filter values in [1]; add is read only where p.addend is
+// set, lo and hi only where their condition holds.  The caller stores z (and y where training keeps it).
+template <int V>
+__device__ __forceinline__ void fd_epi_gate(const FdTapGemm& p, int t, float (&g)[V], float (&f)[V], float (&z)[V],
+                                            const float (&bias)[2][V], const float (&add)[2][V],
+                                            const float (&lo)[2][V], const float (&hi)[2][V]) {
 #pragma unroll
   for (int i = 0; i < V; ++i) {
-    float yg = g[i] * p.acc_scale + full_g[i];
-    float yf = f[i] * p.acc_scale + full_f[i];
-    if (p.addend != nullptr) { yg += ag[i]; yf += af[i]; }
-    if (e_lo) { yg -= lo_g[i]; yf -= lo_f[i]; }
-    if (e_hi) { yg -= hi_g[i]; yf -= hi_f[i]; }
-    yg8[i] = yg; yf8[i] = yf;
-    z[i] = fd_sigmoid(yg) * fd_tanh(yf);
+    g[i] = g[i] * p.acc_scale + bias[0][i];
+    f[i] = f[i] * p.acc_scale + bias[1][i];
   }
-  if (p.y_planes != nullptr) {   // training: keep the pre-activations (packed column order: gates | filters per tile)
-    const int half = p.gate_tile / 2;
-    const int ng = (zc0 / half) * p.gate_tile + (zc0 % half);
-    const size_t yplane = (size_t)p.B * p.T * p.n_total;
-    const size_t yoff = ((size_t)b * p.T + t) * p.n_total;
-    fd_store_planes<V>(p.y_planes, yplane, yoff + ng, yg8, prec);
-    fd_store_planes<V>(p.y_planes, yplane, yoff + ng + half, yf8, prec);
+  if (p.addend != nullptr) {
+#pragma unroll
+    for (int i = 0; i < V; ++i) { g[i] += add[0][i]; f[i] += add[1][i]; }
   }
-  const size_t plane_elems = (size_t)p.B * p.T * p.C;
-  const size_t off = ((size_t)b * p.T + t) * p.C + zc0;
-  fd_store_planes<V>(p.out_planes, plane_elems, off, z, prec);
+  if (t < p.dil) {
+#pragma unroll
+    for (int i = 0; i < V; ++i) { g[i] -= lo[0][i]; f[i] -= lo[1][i]; }
+  }
+  if (t + p.dil >= p.T) {
+#pragma unroll
+    for (int i = 0; i < V; ++i) { g[i] -= hi[0][i]; f[i] -= hi[1][i]; }
+  }
+#pragma unroll
+  for (int i = 0; i < V; ++i) z[i] = fd_sigmoid(g[i]) * fd_tanh(f[i]);
 }
 
+// GATE_BWD's column sums of dy over a lane's rows (gate columns in [0], filter columns in [1]): over all its rows, and
+// over those among the first / last `dil` steps of the item
+template <int V>
+struct FdColSums {
+  float all[2][V], lo[2][V], hi[2][V];
+};
+
+// GATE_BWD (training): the accumulators are dz at channels [n, n + V) (n_total = C).  With the saved pre-activations
+// y_planes [2][B][T][2C] (packed order) the fragment's rows get dy = (dz tanh(f) sg (1-sg) | dz sg (1-tanh(f)^2)) in
+// out_planes, and s (zero on entry) collects the column sums of dy.  All loads are issued before the first store.
+template <int R, int V, int PREC, typename I>
+__device__ __forceinline__ void fd_epi_gate_bwd(const FdTapGemm& p, const FdRows<I>& rw, int n, const float (&a)[R][V],
+                                                FdColSums<V>& s) {
+  const int prec = PREC < 0 ? p.prec : PREC;
+  const int half = p.gate_tile / 2;
+  const I w2 = 2 * (I)p.C, pg = (I)fd_gate_col(p, n);
+  const size_t plane = (size_t)p.B * p.T * w2;
+  I off[R];
+  float g[R][V], f[R][V];
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    off[r] = rw.row(p, r) * w2 + pg;
+    fd_load_planes<V>(p.y_planes, plane, off[r], g[r], prec);
+    fd_load_planes<V>(p.y_planes, plane, off[r] + half, f[r], prec);
+  }
+  const bool sums = p.cs != nullptr || p.cs_edge != nullptr;
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    if (r >= rw.nrows) break;
+    float dg[V], df[V];
+#pragma unroll
+    for (int i = 0; i < V; ++i) fd_dgate(a[r][i] * p.acc_scale, g[r][i], f[r][i], dg[i], df[i]);
+    fd_store_planes<V>(p.out_planes, plane, off[r], dg, prec);
+    fd_store_planes<V>(p.out_planes, plane, off[r] + half, df, prec);
+    if (sums) {
+      const int t = rw.t0 + r * rw.dt;
+      const bool in_lo = t < p.dil, in_hi = t + p.dil >= p.T;
+#pragma unroll
+      for (int i = 0; i < V; ++i) {
+        s.all[0][i] += dg[i]; s.all[1][i] += df[i];
+        if (in_lo) { s.lo[0][i] += dg[i]; s.lo[1][i] += df[i]; }
+        if (in_hi) { s.hi[0][i] += dg[i]; s.hi[1][i] += df[i]; }
+      }
+    }
+  }
+}
+
+// GATE_BWD's column sums of item b, channels [n, n + V): the lanes lane ^ FIRST_XOR, lane ^ 2 FIRST_XOR, ... hold the
+// same columns and are summed by an xor butterfly, then the lanes with `lead` add one atomic per column to cs and,
+// where the warp's rows hold edge steps (warp-uniform edge_lo / edge_hi), to cs_edge.  Every lane of the warp calls it.
+template <int FIRST_XOR, int V>
+__device__ __forceinline__ void fd_gate_bwd_colsums(const FdTapGemm& p, FdColSums<V>& s, bool edge_lo, bool edge_hi,
+                                                    bool lead, int b, int n) {
+  if (p.cs == nullptr && p.cs_edge == nullptr) return;
+  auto butterfly = [](float (&x)[2][V], int i) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int o = FIRST_XOR; o < 32; o *= 2) x[h][i] += __shfl_xor_sync(0xffffffffu, x[h][i], o);
+  };
+#pragma unroll
+  for (int i = 0; i < V; ++i) {
+    butterfly(s.all, i);
+    if (edge_lo) butterfly(s.lo, i);
+    if (edge_hi) butterfly(s.hi, i);
+  }
+  if (!lead) return;
+  const int half = p.gate_tile / 2;
+  const size_t w2 = 2 * (size_t)p.C, c = (size_t)b * w2 + fd_gate_col(p, n);
+  if (p.cs != nullptr) {
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+      atomicAdd(p.cs + c + i, s.all[0][i] * p.cs_scale);
+      atomicAdd(p.cs + c + half + i, s.all[1][i] * p.cs_scale);
+    }
+  }
+  if (p.cs_edge != nullptr && (edge_lo || edge_hi)) {
+    float* const e0 = p.cs_edge + c;
+    float* const e1 = e0 + (size_t)p.B * w2;
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+      if (edge_lo) { atomicAdd(e0 + i, s.lo[0][i] * p.cs_scale); atomicAdd(e0 + half + i, s.lo[1][i] * p.cs_scale); }
+      if (edge_hi) { atomicAdd(e1 + i, s.hi[0][i] * p.cs_scale); atomicAdd(e1 + half + i, s.hi[1][i] * p.cs_scale); }
+    }
+  }
+}
+
+// MAG (framed DFT): V real and V imaginary accumulators of row t, magnitudes of channels [zc0, zc0 + V)
 template <int V, int PREC = -1>
 __device__ __forceinline__ void fd_epi_mag(const FdTapGemm& p, int b, int t, int zc0,
                                            const float (&re)[V], const float (&im)[V]) {
@@ -415,41 +562,6 @@ __device__ __forceinline__ void fd_epi_mag(const FdTapGemm& p, int b, int t, int
   const size_t plane_elems = (size_t)p.B * p.T * p.C;
   const size_t off = ((size_t)b * p.T + t) * p.C + zc0;
   fd_store_planes<V>(p.out_planes, plane_elems, off, z, prec);
-}
-
-// residual/skip epilogue for V consecutive packed columns [n0, n0+V) (n0 < C: residual, else skip)
-template <int V, int PREC = -1>
-__device__ __forceinline__ void fd_epi_res_skip(const FdTapGemm& p, int b, int t, int n0,
-                                                const float (&acc)[V], const float* bias /*indexed by i*/) {
-  const int prec = PREC < 0 ? p.prec : PREC;   // compile-time in the tensor-core kernel
-  const size_t row = (size_t)b * p.T + t;
-  const size_t plane_elems = (size_t)p.B * p.T * p.C;
-  float y[V];
-#pragma unroll
-  for (int i = 0; i < V; ++i) y[i] = acc[i] * p.acc_scale + bias[i];
-  if (n0 < p.C) {
-    if (p.last_layer) return;  // the residual stream is not consumed after the last layer
-    const size_t off = row * p.C + n0;
-    float x[V];
-    fd_load_planes<V>(p.x_planes, plane_elems, off, x, prec);
-#pragma unroll
-    for (int i = 0; i < V; ++i) x[i] = (x[i] + y[i]) * 0.70710678118654752440f;
-    fd_store_planes<V>(p.x_out_planes != nullptr ? p.x_out_planes : p.x_planes, plane_elems, off, x, prec);
-  } else {
-    const size_t off = row * p.C + (n0 - p.C);
-    if (!p.first_layer) {
-      float s[V]; fd_load_f32<V>(p.skip_f32 + off, s);
-#pragma unroll
-      for (int i = 0; i < V; ++i) y[i] += s[i];
-    }
-    if (p.last_layer) {
-#pragma unroll
-      for (int i = 0; i < V; ++i) y[i] *= p.skip_scale;
-      fd_store_planes<V>(p.skip_planes, plane_elems, off, y, prec);
-    } else {
-      fd_store_f32<V>(p.skip_f32 + off, y);
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,8 +1,8 @@
-// SIMT fp32 twins of the tap-GEMM (same operands, same packed weights, same epilogues as the
-// wgmma kernel in fd_tapgemm_tc.cu) and of the weight-gradient GEMM (fd_wgrad_tc.cu).  They exist
-// (a) as the device-side check of the tensor-core kernels, (b) for shapes the tensor-core
-// instantiations do not cover.  They are plain CUDA-core FFMA over (hi+lo) recombined operands,
-// i.e. fp32 arithmetic on 22-bit (f16 planes) inputs.
+// SIMT fp32 twins of the tap-GEMM (same operands and packed weights as the wgmma kernels in fd_tapgemm_tc.cu, and the
+// same epilogue definitions from fd_common.cuh, called on fragments of RM rows x 4 columns: one per column group) and
+// of the weight-gradient GEMM (fd_wgrad_tc.cu).  They exist (a) as the device-side check of the tensor-core kernels,
+// (b) for shapes the tensor-core instantiations do not cover.  They are plain CUDA-core FFMA over (hi+lo) recombined
+// operands, i.e. fp32 arithmetic on 22-bit (f16 planes) inputs.
 #include "fd_common.cuh"
 
 namespace {
@@ -32,10 +32,8 @@ __global__ void __launch_bounds__(256) fd_tapgemm_simt_kernel(const FdTapGemm p)
 
   int run0, run1;
   if (EPI == FD_EPI_GATE || EPI == FD_EPI_MAG) {
-    const int half = p.gate_tile / 2;
-    const int zc0 = j * RUN;
-    run0 = (zc0 / half) * p.gate_tile + (zc0 % half);
-    run1 = run0 + half;
+    run0 = fd_gate_col(p, j * RUN);
+    run1 = run0 + p.gate_tile / 2;
   } else {
     run0 = j * BN;
     run1 = run0 + RUN;
@@ -109,82 +107,69 @@ __global__ void __launch_bounds__(256) fd_tapgemm_simt_kernel(const FdTapGemm p)
     koff += sg.k_len;
   }
 
-  // ---- epilogue
-  if constexpr (EPI == FD_EPI_GATE_BWD) {
-    // the accumulators are dz: dy of this thread's two 4-column groups, each gate group with its filter group half a
-    // tile further on, and the column sums of dy over this thread's rows
-    const int half = p.gate_tile / 2;
-    const size_t W2 = 2 * (size_t)p.C, plane = (size_t)p.B * p.T * W2;
-    const bool edge0 = t0 < p.dil, edge1 = t0 + BM + p.dil > p.T;   // CTA-uniform: the tile holds edge rows
+  // ---- epilogue: this thread's rows t0 + ty RM .. + RM - 1, one at a time, in two 4-column groups (gate and filter
+  //      columns for GATE / MAG, whose definitions take both)
+  const int tr = t0 + ty * RM, nrows = max(0, min(RM, p.T - tr));
+  if constexpr (EPI == FD_EPI_GATE || EPI == FD_EPI_MAG) {
+    const int zc = j * RUN + tx * 4, n_g = run0 + tx * 4, n_f = run1 + tx * 4;
+    if (n_g >= p.n_total) return;
+    const size_t zplane = (size_t)p.B * p.T * p.C, yplane = (size_t)p.B * p.T * p.n_total;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int n = (h == 0 ? run0 : run1) + tx * 4;
-      const int pg = (n / half) * p.gate_tile + n % half;
-      float cs[8] = {}, e0[8] = {}, e1[8] = {};     // sums of dg (0..3) and df (4..7)
-#pragma unroll
-      for (int r = 0; r < RM; ++r) {
-        const int t = t0 + ty * RM + r;
-        if (t >= p.T || n >= p.n_total) continue;
-        const size_t off = ((size_t)b * p.T + t) * W2 + pg;
-        float g[4], f[4], dg[4], df[4];
-        fd_load_planes<4>(p.y_planes, plane, off, g, p.prec);
-        fd_load_planes<4>(p.y_planes, plane, off + half, f, p.prec);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) fd_dgate(acc[r][4 * h + i] * p.acc_scale, g[i], f[i], dg[i], df[i]);
-        fd_store_planes<4>(p.out_planes, plane, off, dg, p.prec);
-        fd_store_planes<4>(p.out_planes, plane, off + half, df, p.prec);
+    for (int r = 0; r < RM; ++r) {
+      if (r >= nrows) break;
+      const int t = tr + r;
+      float g[4] = {acc[r][0], acc[r][1], acc[r][2], acc[r][3]};
+      float f[4] = {acc[r][4], acc[r][5], acc[r][6], acc[r][7]};
+      if constexpr (EPI == FD_EPI_MAG) {
+        fd_epi_mag<4>(p, b, t, zc, g, f);
+      } else {
+        const size_t row = (size_t)b * p.T + t, bo = (size_t)b * p.gbias_bstride;
+        float add[2][4], bias[2][4], lo[2][4], hi[2][4], z[4];
+        if (p.addend != nullptr) {
+          fd_load_f32<4>(p.addend + row * p.n_total + n_g, add[0]);
+          fd_load_f32<4>(p.addend + row * p.n_total + n_f, add[1]);
+        }
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          cs[i] += dg[i]; cs[4 + i] += df[i];
-          if (t < p.dil) { e0[i] += dg[i]; e0[4 + i] += df[i]; }
-          if (t + p.dil >= p.T) { e1[i] += dg[i]; e1[4 + i] += df[i]; }
+          bias[0][i] = p.gbias_full[bo + n_g + i]; bias[1][i] = p.gbias_full[bo + n_f + i];
+          lo[0][i] = p.gbias_lo[bo + n_g + i]; lo[1][i] = p.gbias_lo[bo + n_f + i];
+          hi[0][i] = p.gbias_hi[bo + n_g + i]; hi[1][i] = p.gbias_hi[bo + n_f + i];
         }
-      }
-      // the lanes of a warp with this tx hold the same columns: sum over them, then one atomic per column and warp
-#pragma unroll
-      for (int o = TXC; o < 32; o *= 2)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          cs[i] += __shfl_xor_sync(0xffffffffu, cs[i], o);
-          if (edge0) e0[i] += __shfl_xor_sync(0xffffffffu, e0[i], o);
-          if (edge1) e1[i] += __shfl_xor_sync(0xffffffffu, e1[i], o);
+        fd_epi_gate<4>(p, t, g, f, z, bias, add, lo, hi);
+        if (p.y_planes != nullptr) {   // training: keep the pre-activations
+          fd_store_planes<4>(p.y_planes, yplane, row * p.n_total + n_g, g, p.prec);
+          fd_store_planes<4>(p.y_planes, yplane, row * p.n_total + n_f, f, p.prec);
         }
-      if (tid % 32 >= TXC || n >= p.n_total) continue;
-      const size_t co = (size_t)b * W2 + pg;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const size_t c = co + (i < 4 ? i : half + i - 4);
-        if (p.cs != nullptr) atomicAdd(p.cs + c, cs[i] * p.cs_scale);
-        if (p.cs_edge != nullptr && edge0) atomicAdd(p.cs_edge + c, e0[i] * p.cs_scale);
-        if (p.cs_edge != nullptr && edge1) atomicAdd(p.cs_edge + (size_t)p.B * W2 + c, e1[i] * p.cs_scale);
+        fd_store_planes<4>(p.out_planes, zplane, row * p.C + zc, z, p.prec);
       }
     }
   } else {
 #pragma unroll
-    for (int r = 0; r < RM; ++r) {
-      const int t = t0 + ty * RM + r;
-      if (t >= p.T) continue;
-      float v0[4] = {acc[r][0], acc[r][1], acc[r][2], acc[r][3]};
-      float v1[4] = {acc[r][4], acc[r][5], acc[r][6], acc[r][7]};
-      const int n_a = run0 + tx * 4, n_b = run1 + tx * 4;
-      if (EPI == FD_EPI_LINEAR) {
-        const float* bias = p.bias ? p.bias + (size_t)b * p.bias_bstride : nullptr;
-        if (n_a < p.n_total) fd_epi_linear<4>(p, b, t, n_a, v0, bias, 0);
-        if (n_b < p.n_total) fd_epi_linear<4>(p, b, t, n_b, v1, bias, 0);
-      } else if (EPI == FD_EPI_GATE) {
-        if (n_a < p.n_total) {
-          const size_t bo = (size_t)b * p.gbias_bstride;
-          fd_epi_gate<4>(p, b, t, j * RUN + tx * 4, n_a, n_b, v0, v1,
-                         p.gbias_full + bo + n_a, p.gbias_full + bo + n_b,
-                         p.gbias_lo + bo + n_a, p.gbias_lo + bo + n_b,
-                         p.gbias_hi + bo + n_a, p.gbias_hi + bo + n_b);
+    for (int h = 0; h < 2; ++h) {
+      const int n = (h == 0 ? run0 : run1) + tx * 4;
+      if constexpr (EPI == FD_EPI_GATE_BWD) {
+        // the lanes of a warp with this tx hold the same columns; the edge flags are CTA-uniform
+        FdColSums<4> s{};
+#pragma unroll
+        for (int r = 0; r < RM; ++r) {
+          if (r >= nrows || n >= p.n_total) break;
+          float a[1][4] = {{acc[r][4 * h], acc[r][4 * h + 1], acc[r][4 * h + 2], acc[r][4 * h + 3]}};
+          fd_epi_gate_bwd<1, 4, -1>(p, FdRows<size_t>{(size_t)b * p.T, tr + r, 1, 1}, n, a, s);
         }
-      } else if (EPI == FD_EPI_MAG) {
-        if (n_a < p.n_total) fd_epi_mag<4>(p, b, t, j * RUN + tx * 4, v0, v1);
+        fd_gate_bwd_colsums<TXC>(p, s, t0 < p.dil, t0 + BM + p.dil > p.T, tid % 32 < TXC && n < p.n_total, b, n);
       } else {
-        const float* bias = p.bias + (size_t)b * p.bias_bstride;
-        if (n_a < p.n_total) fd_epi_res_skip<4>(p, b, t, n_a, v0, bias + n_a);
-        if (n_b < p.n_total) fd_epi_res_skip<4>(p, b, t, n_b, v1, bias + n_b);
+        if (n >= p.n_total) continue;
+#pragma unroll
+        for (int r = 0; r < RM; ++r) {
+          if (r >= nrows) break;
+          float bias[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) bias[i] = p.bias != nullptr ? p.bias[(size_t)b * p.bias_bstride + n + i] : 0.f;
+          float a[1][4] = {{acc[r][4 * h], acc[r][4 * h + 1], acc[r][4 * h + 2], acc[r][4 * h + 3]}};
+          const FdRows<size_t> row{(size_t)b * p.T, tr + r, 1, 1};
+          if constexpr (EPI == FD_EPI_LINEAR) fd_epi_linear<1, 4, -1>(p, row, n, a, bias);
+          else fd_epi_res_skip<1, 4, -1>(p, row, n, n < p.C, a, bias);
+        }
       }
     }
   }

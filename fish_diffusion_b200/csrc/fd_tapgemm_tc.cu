@@ -87,7 +87,7 @@ template <int BLOCK_N, int EPI, int PREC>
 __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* acc, int b, int n_tile, int rw0,
                                               const float* bias_s, uint32_t my_scratch, int lane) {
   const int n0 = n_tile * BLOCK_N;
-  if (EPI == FD_EPI_GATE || EPI == FD_EPI_MAG) {
+  if constexpr (EPI == FD_EPI_GATE || EPI == FD_EPI_MAG) {
     // 16 gate columns and the matching 16 filter columns per step; lane -> row lane/2, 8 columns (lane % 2)
     constexpr int HALF = BLOCK_N / 2;       // gate columns | filter columns
     const uint32_t sb = smem_u32(bias_s);
@@ -98,7 +98,6 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
     const bool edge_any = __any_sync(0xffffffffu, valid && (e_lo || e_hi));
     const size_t zplane = (size_t)p.B * p.T * p.C, zrow = ((size_t)b * p.T + t) * p.C + (size_t)n_tile * HALF;
     const size_t yplane = (size_t)p.B * p.T * p.n_total, yrow = ((size_t)b * p.T + t) * p.n_total;
-    const int halfg = p.gate_tile / 2;
 #pragma unroll
     for (int c = 0; c < HALF; c += 16) {
       frag_to_scratch<16>(my_scratch, acc, c, 0, lane);
@@ -117,308 +116,72 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
         if (EPI == FD_EPI_MAG) {
           fd_epi_mag<8, PREC>(p, b, t, n_tile * HALF + cc, g, f);
         } else {
-          // the bias vectors are read with shared-space loads, and the zero-padding corrections of the first / last
-          // `dilation` rows are skipped by a warp vote where no lane needs them
-          float yg[8], yf[8], z[8];
-          {
-            // the addend (conditioner projection, packed columns n0 + cc and n0 + HALF + cc of this row) is issued
-            // with the bias loads; it is read once per launch, so it streams past L2 (evict-first)
-            float4 c0, c1, d0, d1;
-            if (p.addend != nullptr) {
-              const float* ad = p.addend + yrow + n0 + cc;
-              c0 = __ldcs(reinterpret_cast<const float4*>(ad));
-              c1 = __ldcs(reinterpret_cast<const float4*>(ad + 4));
-              d0 = __ldcs(reinterpret_cast<const float4*>(ad + HALF));
-              d1 = __ldcs(reinterpret_cast<const float4*>(ad + HALF + 4));
-            }
-            const float4 a0 = lds128(sb + 4u * cc), a1 = lds128(sb + 4u * cc + 16u);
-            const float4 b0 = lds128(sb + 4u * (HALF + cc)), b1 = lds128(sb + 4u * (HALF + cc) + 16u);
-            const float bg[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const float bf[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+          // the addend (conditioner projection, packed columns n0 + cc and n0 + HALF + cc of this row) is issued before
+          // the shared-space bias loads; it is read once per launch, so it streams past L2 (evict-first).  The
+          // zero-padding corrections of the first / last `dilation` rows are skipped by a warp vote where no lane
+          // needs them.
+          float add[2][8], bias[2][8], lo[2][8], hi[2][8], z[8];
+          if (p.addend != nullptr) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              yg[i] = g[i] * p.acc_scale + bg[i];
-              yf[i] = f[i] * p.acc_scale + bf[i];
-            }
-            if (p.addend != nullptr) {
-              const float cg[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-              const float cf[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-#pragma unroll
-              for (int i = 0; i < 8; ++i) { yg[i] += cg[i]; yf[i] += cf[i]; }
-            }
+            for (int h = 0; h < 2; ++h) ldcs_f32(p.addend + yrow + n0 + h * HALF + cc, add[h]);
           }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) lds_f32(sb + 4u * (h * HALF + cc), bias[h]);
           if (edge_any) {
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              if (e == 0 ? e_lo : e_hi) {
-                const uint32_t eb = sb + 4u * ((1 + e) * BLOCK_N + cc);
-                const float4 a0 = lds128(eb), a1 = lds128(eb + 16u);
-                const float4 b0 = lds128(eb + 4u * HALF), b1 = lds128(eb + 4u * HALF + 16u);
-                const float eg[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                const float ef[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+            for (int h = 0; h < 2; ++h)
+              if (e_lo) lds_f32(sb + 4u * (BLOCK_N + h * HALF + cc), lo[h]);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) { yg[i] -= eg[i]; yf[i] -= ef[i]; }
-              }
-            }
+            for (int h = 0; h < 2; ++h)
+              if (e_hi) lds_f32(sb + 4u * (2 * BLOCK_N + h * HALF + cc), hi[h]);
           }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) z[i] = fd_sigmoid(yg[i]) * fd_tanh(yf[i]);
+          fd_epi_gate<8>(p, t, g, f, z, bias, add, lo, hi);
           if (p.y_planes != nullptr) {   // training: keep the pre-activations (packed column order: gates | filters per tile)
-            const int zc0 = n_tile * HALF + cc;
-            const int ng = p.gate_tile == BLOCK_N ? n_tile * BLOCK_N + cc : (zc0 / halfg) * p.gate_tile + (zc0 % halfg);
-            fd_store_planes<8>(p.y_planes, yplane, yrow + ng, yg, PREC);
-            fd_store_planes<8>(p.y_planes, yplane, yrow + ng + halfg, yf, PREC);
+            const int ng = p.gate_tile == BLOCK_N ? n0 + cc : fd_gate_col(p, n_tile * HALF + cc);
+            fd_store_planes<8>(p.y_planes, yplane, yrow + ng, g, PREC);
+            fd_store_planes<8>(p.y_planes, yplane, yrow + ng + p.gate_tile / 2, f, PREC);
           }
           fd_store_planes<8>(p.out_planes, zplane, zrow + cc, z, PREC);
         }
       }
     }
-  } else if (BLOCK_N >= 64) {
-    // ---- LINEAR / RES_SKIP / GATE_BWD, coalescing epilogue: 32-column chunks; lane -> rows rbase + 4 pp (pp < 4),
+  } else if constexpr (BLOCK_N >= 64) {
+    // ---- LINEAR / RES_SKIP / GATE_BWD, coalescing epilogue: 32-column chunks; lane -> rows rbase + 4 r (r < 4),
     //      columns 4 (lane % 8) .. + 3 of the chunk, so that 8 lanes cover one 128-byte row segment
     const uint32_t bias_addr = smem_u32(bias_s);
     const int j4 = (lane & 7) * 4, rsub = lane >> 3;
-    const int rbase = rw0 + rsub;                      // time index of pass 0
-    const int nrows = rbase < p.T ? min(4, (p.T - rbase + 3) / 4) : 0;   // rows rbase + 4 pp < T
-    const uint32_t rowbase = (uint32_t)b * (uint32_t)p.T;
+    const int rbase = rw0 + rsub;                      // time index of row 0
+    const FdRows<uint32_t> rows{(uint32_t)b * (uint32_t)p.T, rbase, 4,
+                                rbase < p.T ? min(4, (p.T - rbase + 3) / 4) : 0};
 #pragma unroll
     for (int c = 0; c < BLOCK_N; c += 32) {
       const int col = c + j4;                          // first of this lane's 4 columns inside the tile
       const int n = n0 + col;                          // global packed column
       frag_to_scratch<32>(my_scratch, acc, c, 0, lane);
       __syncwarp();
-      float4 a[4];
+      float a[4][4];
 #pragma unroll
-      for (int pp = 0; pp < 4; ++pp) a[pp] = scratch_ld4(my_scratch, 4 * pp + rsub, lane & 7);
+      for (int r = 0; r < 4; ++r) {
+        const float4 x = scratch_ld4(my_scratch, 4 * r + rsub, lane & 7);
+        a[r][0] = x.x; a[r][1] = x.y; a[r][2] = x.z; a[r][3] = x.w;
+      }
       __syncwarp();
-      if (EPI == FD_EPI_GATE_BWD) {
-        // backward of z = sigmoid(g) tanh(f) fused into the dz GEMM (training): this lane's 4 channels n..n+3 of 4 rows
-        const int half_g = p.gate_tile / 2;
-        const uint32_t pg = (uint32_t)((n / half_g) * p.gate_tile + (n % half_g));     // packed gate column
-        const uint32_t W2 = 2u * (uint32_t)p.C;
-        const size_t yplane = (size_t)p.B * p.T * W2;
-        const uint16_t* const y_lo = p.y_planes + yplane;
-        uint16_t* const o_lo = p.out_planes + yplane;
-        float sg4[4] = {0.f, 0.f, 0.f, 0.f}, sf4[4] = {0.f, 0.f, 0.f, 0.f};          // column sums over this lane's rows
-        float e0g[4] = {0.f, 0.f, 0.f, 0.f}, e0f[4] = {0.f, 0.f, 0.f, 0.f}, e1g[4] = {0.f, 0.f, 0.f, 0.f}, e1f[4] = {0.f, 0.f, 0.f, 0.f};
-        uint2 gh[4], gl[4], fh[4], fl[4];
-        uint32_t eo4[4];
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) {
-          eo4[pp] = (rowbase + (uint32_t)min(rbase + pp * 4, p.T - 1)) * W2 + pg;
-          gh[pp] = *reinterpret_cast<const uint2*>(p.y_planes + eo4[pp]);
-          gl[pp] = *reinterpret_cast<const uint2*>(y_lo + eo4[pp]);
-          fh[pp] = *reinterpret_cast<const uint2*>(p.y_planes + eo4[pp] + half_g);
-          fl[pp] = *reinterpret_cast<const uint2*>(y_lo + eo4[pp] + half_g);
-        }
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) {
-          if (pp >= nrows) break;
-          float g[4], f[4];
-          fd_combine2(gh[pp].x, gl[pp].x, PREC, g[0], g[1]);
-          fd_combine2(gh[pp].y, gl[pp].y, PREC, g[2], g[3]);
-          fd_combine2(fh[pp].x, fl[pp].x, PREC, f[0], f[1]);
-          fd_combine2(fh[pp].y, fl[pp].y, PREC, f[2], f[3]);
-          const float dzv[4] = {a[pp].x * p.acc_scale, a[pp].y * p.acc_scale, a[pp].z * p.acc_scale, a[pp].w * p.acc_scale};
-          float dg[4], df[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) fd_dgate(dzv[i], g[i], f[i], dg[i], df[i]);
-          uint32_t h0, l0, h1, l1;
-          fd_split2(dg[0], dg[1], PREC, h0, l0);
-          fd_split2(dg[2], dg[3], PREC, h1, l1);
-          *reinterpret_cast<uint2*>(p.out_planes + eo4[pp]) = make_uint2(h0, h1);
-          *reinterpret_cast<uint2*>(o_lo + eo4[pp]) = make_uint2(l0, l1);
-          fd_split2(df[0], df[1], PREC, h0, l0);
-          fd_split2(df[2], df[3], PREC, h1, l1);
-          *reinterpret_cast<uint2*>(p.out_planes + eo4[pp] + half_g) = make_uint2(h0, h1);
-          *reinterpret_cast<uint2*>(o_lo + eo4[pp] + half_g) = make_uint2(l0, l1);
-          if (p.cs != nullptr) {
-            const int tt = rbase + pp * 4;
-            const bool in0 = tt < p.dil, in1 = tt + p.dil >= p.T;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              sg4[i] += dg[i]; sf4[i] += df[i];
-              if (in0) { e0g[i] += dg[i]; e0f[i] += df[i]; }
-              if (in1) { e1g[i] += dg[i]; e1f[i] += df[i]; }
-            }
-          }
-        }
-        if (p.cs != nullptr) {
-          // rows of the 4 lanes that share these columns (lane bits 3,4), then one atomic per column and warp
-          const bool edge0 = rw0 < p.dil, edge1 = rw0 + 16 + p.dil > p.T;     // warp-uniform
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            sg4[i] += __shfl_xor_sync(0xffffffffu, sg4[i], 8); sg4[i] += __shfl_xor_sync(0xffffffffu, sg4[i], 16);
-            sf4[i] += __shfl_xor_sync(0xffffffffu, sf4[i], 8); sf4[i] += __shfl_xor_sync(0xffffffffu, sf4[i], 16);
-            if (edge0) {
-              e0g[i] += __shfl_xor_sync(0xffffffffu, e0g[i], 8); e0g[i] += __shfl_xor_sync(0xffffffffu, e0g[i], 16);
-              e0f[i] += __shfl_xor_sync(0xffffffffu, e0f[i], 8); e0f[i] += __shfl_xor_sync(0xffffffffu, e0f[i], 16);
-            }
-            if (edge1) {
-              e1g[i] += __shfl_xor_sync(0xffffffffu, e1g[i], 8); e1g[i] += __shfl_xor_sync(0xffffffffu, e1g[i], 16);
-              e1f[i] += __shfl_xor_sync(0xffffffffu, e1f[i], 8); e1f[i] += __shfl_xor_sync(0xffffffffu, e1f[i], 16);
-            }
-          }
-          if (rsub == 0) {
-            float* const csb = p.cs + (size_t)b * W2 + pg;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              atomicAdd(csb + i, sg4[i] * p.cs_scale);
-              atomicAdd(csb + half_g + i, sf4[i] * p.cs_scale);
-            }
-            if (p.cs_edge != nullptr && (edge0 || edge1)) {
-              float* const ce0 = p.cs_edge + (size_t)b * W2 + pg;
-              float* const ce1 = ce0 + (size_t)p.B * W2;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                if (edge0) { atomicAdd(ce0 + i, e0g[i] * p.cs_scale); atomicAdd(ce0 + half_g + i, e0f[i] * p.cs_scale); }
-                if (edge1) { atomicAdd(ce1 + i, e1g[i] * p.cs_scale); atomicAdd(ce1 + half_g + i, e1f[i] * p.cs_scale); }
-              }
-            }
-          }
-        }
-      } else if (EPI == FD_EPI_RES_SKIP) {
-        // residual columns: x' = (x + y)/sqrt2 on the split planes; skip columns: fp32 accumulation.  32-bit element
-        // offsets (checked on the host), rows past T clamped for the loads and skipped for the stores.
-        const float4 bias4 = lds128(bias_addr + 4u * col);
-        const bool is_res = n0 < p.C;
-        const uint32_t cn = (uint32_t)(is_res ? n : n - p.C);
-        const size_t plane = (size_t)p.B * p.T * p.C;
-        uint32_t eo[4];
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp)
-          eo[pp] = (rowbase + (uint32_t)min(rbase + pp * 4, p.T - 1)) * (uint32_t)p.C + cn;
-        if (is_res) {
-          if (!p.last_layer) {
-            const uint16_t* const xlo = p.x_planes + plane;
-            uint16_t* const xo = p.x_out_planes != nullptr ? p.x_out_planes : p.x_planes;
-            uint16_t* const xo_lo = xo + plane;
-            uint2 h2[4], l2[4];
-#pragma unroll
-            for (int pp = 0; pp < 4; ++pp) {
-              h2[pp] = *reinterpret_cast<const uint2*>(p.x_planes + eo[pp]);
-              l2[pp] = *reinterpret_cast<const uint2*>(xlo + eo[pp]);
-            }
-#pragma unroll
-            for (int pp = 0; pp < 4; ++pp) {
-              if (pp >= nrows) break;
-              float x0, x1, x2, x3;
-              fd_combine2(h2[pp].x, l2[pp].x, PREC, x0, x1);
-              fd_combine2(h2[pp].y, l2[pp].y, PREC, x2, x3);
-              x0 = (x0 + (a[pp].x * p.acc_scale + bias4.x)) * 0.70710678118654752440f;
-              x1 = (x1 + (a[pp].y * p.acc_scale + bias4.y)) * 0.70710678118654752440f;
-              x2 = (x2 + (a[pp].z * p.acc_scale + bias4.z)) * 0.70710678118654752440f;
-              x3 = (x3 + (a[pp].w * p.acc_scale + bias4.w)) * 0.70710678118654752440f;
-              uint32_t h0, l0, h1, l1;
-              fd_split2(x0, x1, PREC, h0, l0);
-              fd_split2(x2, x3, PREC, h1, l1);
-              *reinterpret_cast<uint2*>(xo + eo[pp]) = make_uint2(h0, h1);
-              *reinterpret_cast<uint2*>(xo_lo + eo[pp]) = make_uint2(l0, l1);
-            }
-          }
-        } else {
-          float4 sk[4];
-          if (!p.first_layer) {
-#pragma unroll
-            for (int pp = 0; pp < 4; ++pp) sk[pp] = *reinterpret_cast<const float4*>(p.skip_f32 + eo[pp]);
-          }
-          uint16_t* const sk_lo = p.skip_planes + plane;
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            if (pp >= nrows) break;
-            float y0 = a[pp].x * p.acc_scale + bias4.x, y1 = a[pp].y * p.acc_scale + bias4.y;
-            float y2 = a[pp].z * p.acc_scale + bias4.z, y3 = a[pp].w * p.acc_scale + bias4.w;
-            if (!p.first_layer) { y0 += sk[pp].x; y1 += sk[pp].y; y2 += sk[pp].z; y3 += sk[pp].w; }
-            if (p.last_layer) {
-              uint32_t h0, l0, h1, l1;
-              fd_split2(y0 * p.skip_scale, y1 * p.skip_scale, PREC, h0, l0);
-              fd_split2(y2 * p.skip_scale, y3 * p.skip_scale, PREC, h1, l1);
-              *reinterpret_cast<uint2*>(p.skip_planes + eo[pp]) = make_uint2(h0, h1);
-              *reinterpret_cast<uint2*>(sk_lo + eo[pp]) = make_uint2(l0, l1);
-            } else {
-              *reinterpret_cast<float4*>(p.skip_f32 + eo[pp]) = make_float4(y0, y1, y2, y3);
-            }
-          }
-        }
+      if constexpr (EPI == FD_EPI_GATE_BWD) {
+        // the 4 lanes that share these columns are lane bits 3 and 4; the warp's 16 rows decide the edge flags
+        FdColSums<4> s{};
+        fd_epi_gate_bwd<4, 4, PREC>(p, rows, n, a, s);
+        fd_gate_bwd_colsums<8>(p, s, rw0 < p.dil, rw0 + 16 + p.dil > p.T, rsub == 0, b, n);
       } else {
-        // LINEAR (vocoder convs, WaveNet head / tail, data gradients): the operands of a chunk are folded kind by kind
-        // into one pre-sum; element offsets are 32-bit (checked on the host) and rows past T are clamped for the loads
-        // and skipped for the stores.
-        const float4 bias4 = lds128(bias_addr + 4u * col);
-        uint32_t eo[4];                                                     // element offset of this lane's 4 columns
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp)
-          eo[pp] = (rowbase + (uint32_t)min(rbase + pp * 4, p.T - 1)) * (uint32_t)p.n_total + (uint32_t)n;
-        float4 pre[4];
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) pre[pp] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.addend != nullptr) {
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const float4 t4 = *reinterpret_cast<const float4*>(p.addend + eo[pp]);
-            pre[pp].x += t4.x; pre[pp].y += t4.y; pre[pp].z += t4.z; pre[pp].w += t4.w;
-          }
-        }
-        if (p.res_f32 != nullptr) {
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const float4 t4 = *reinterpret_cast<const float4*>(p.res_f32 + eo[pp]);
-            pre[pp].x += t4.x; pre[pp].y += t4.y; pre[pp].z += t4.z; pre[pp].w += t4.w;
-          }
-        }
-        if (p.res_planes != nullptr) {
-          const uint16_t* const lo_base = p.res_planes + (size_t)p.B * p.T * p.n_total;
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const uint2 h2 = *reinterpret_cast<const uint2*>(p.res_planes + eo[pp]);
-            const uint2 l2 = *reinterpret_cast<const uint2*>(lo_base + eo[pp]);
-            float r0, r1, r2, r3;
-            fd_combine2(h2.x, l2.x, PREC, r0, r1);
-            fd_combine2(h2.y, l2.y, PREC, r2, r3);
-            pre[pp].x += p.res_scale * r0; pre[pp].y += p.res_scale * r1;
-            pre[pp].z += p.res_scale * r2; pre[pp].w += p.res_scale * r3;
-          }
-        }
-        uint32_t mkbits = 0;
-        if (p.row_mask != nullptr) {
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp)
-            if (p.row_mask[rowbase + (uint32_t)min(rbase + pp * 4, p.T - 1)] != 0) mkbits |= 1u << pp;
-        }
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) {
-          a[pp].x = (a[pp].x * p.acc_scale + bias4.x + pre[pp].x) * p.post_scale;
-          a[pp].y = (a[pp].y * p.acc_scale + bias4.y + pre[pp].y) * p.post_scale;
-          a[pp].z = (a[pp].z * p.acc_scale + bias4.z + pre[pp].z) * p.post_scale;
-          a[pp].w = (a[pp].w * p.acc_scale + bias4.w + pre[pp].w) * p.post_scale;
-        }
-        if (p.out_f32 != nullptr && p.out_accum) {       // accumulate launches: one more batch of loads
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const float4 o4 = *reinterpret_cast<const float4*>(p.out_f32 + eo[pp]);
-            a[pp].x += o4.x; a[pp].y += o4.y; a[pp].z += o4.z; a[pp].w += o4.w;
-          }
-        }
-        const float slope = p.act == FD_ACT_NONE ? 1.f : p.act == FD_ACT_RELU ? 0.f : p.act_slope;
-        uint16_t* const out_lo = p.out_planes + (size_t)p.B * p.T * p.n_total;
-#pragma unroll
-        for (int pp = 0; pp < 4; ++pp) {
-          if (pp >= nrows) break;
-          if ((mkbits >> pp) & 1u) a[pp] = make_float4(0.f, 0.f, 0.f, 0.f);      // masked row: zeros everywhere
-          if (p.out_f32 != nullptr) *reinterpret_cast<float4*>(p.out_f32 + eo[pp]) = a[pp];
-          if (p.out_planes != nullptr) {
-            uint32_t h0, l0, h1, l1;
-            fd_split2(fd_act(a[pp].x * p.planes_scale, slope), fd_act(a[pp].y * p.planes_scale, slope), PREC, h0, l0);
-            fd_split2(fd_act(a[pp].z * p.planes_scale, slope), fd_act(a[pp].w * p.planes_scale, slope), PREC, h1, l1);
-            *reinterpret_cast<uint2*>(p.out_planes + eo[pp]) = make_uint2(h0, h1);
-            *reinterpret_cast<uint2*>(out_lo + eo[pp]) = make_uint2(l0, l1);
-          }
-        }
+        float bias[4];
+        lds_f32(bias_addr + 4u * col, bias);
+        if constexpr (EPI == FD_EPI_RES_SKIP) fd_epi_res_skip<4, 4, PREC>(p, rows, n, n0 < p.C, a, bias);   // C % BLOCK_N == 0
+        else fd_epi_linear<4, 4, PREC>(p, rows, n, a, bias);
       }
     }
   } else {
-    // ---- LINEAR / RES_SKIP with narrow tiles (BLOCK_N <= 32): row-owner epilogue; lane -> row lane/2,
-    //      BLOCK_N/2 columns (lane % 2)
+    // ---- LINEAR with narrow tiles (BLOCK_N <= 32; pick_cfg gives RES_SKIP and GATE_BWD no tile under 64 columns):
+    //      row-owner epilogue; lane -> row lane/2, BLOCK_N/2 columns (lane % 2) in groups of 8
+    static_assert(EPI == FD_EPI_LINEAR, "narrow tiles: LINEAR only");
     constexpr int PER = BLOCK_N / 2;
     frag_to_scratch<BLOCK_N>(my_scratch, acc, 0, 0, lane);
     __syncwarp();
@@ -431,16 +194,15 @@ __device__ __forceinline__ void tile_epilogue(const FdTapGemm& p, const float* a
     }
     __syncwarp();
     const int t = rw0 + r;
-    if (t < p.T) {
+    const FdRows<uint32_t> row{(uint32_t)b * (uint32_t)p.T, t, 1, t < p.T ? 1 : 0};
 #pragma unroll
-      for (int h = 0; h < PER / 8; ++h) {
-        float v8[8];
+    for (int h = 0; h < PER / 8; ++h) {
+      const int cc = sub * PER + h * 8;
+      float a[1][8], bias[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v8[i] = v[h * 8 + i];
-        const int cc = sub * PER + h * 8;
-        if (EPI == FD_EPI_LINEAR) fd_epi_linear<8, PREC>(p, b, t, n0 + cc, v8, bias_s, n0);
-        else fd_epi_res_skip<8, PREC>(p, b, t, n0 + cc, v8, bias_s + cc);
-      }
+      for (int i = 0; i < 8; ++i) a[0][i] = v[h * 8 + i];
+      lds_f32(smem_u32(bias_s) + 4u * cc, bias);
+      fd_epi_linear<1, 8, PREC>(p, row, n0 + cc, a, bias);
     }
   }
 }
@@ -687,11 +449,11 @@ __device__ __forceinline__ void gate_t_epilogue(const FdTapGemm& p, const float*
                                                 uint32_t my_scratch, int lane) {
   const int half = p.gate_tile / 2;
   const int e = lane >> 2, q4 = lane & 3;
-  const int n_g = (ch / half) * p.gate_tile + ch % half + e, n_f = n_g + half;   // packed columns of rows r, r + 8
+  const int n_g = fd_gate_col(p, ch) + e, n_f = n_g + half;   // packed columns of rows r, r + 8
   const size_t bo = (size_t)b * p.gbias_bstride;
-  const float bg = p.gbias_full[bo + n_g], bf = p.gbias_full[bo + n_f];
-  const float lg = p.gbias_lo[bo + n_g], lf = p.gbias_lo[bo + n_f];
-  const float hg = p.gbias_hi[bo + n_g], hf = p.gbias_hi[bo + n_f];
+  const float bias[2][1] = {{p.gbias_full[bo + n_g]}, {p.gbias_full[bo + n_f]}};
+  const float lo[2][1] = {{p.gbias_lo[bo + n_g]}, {p.gbias_lo[bo + n_f]}};
+  const float hi[2][1] = {{p.gbias_hi[bo + n_g]}, {p.gbias_hi[bo + n_f]}};
   const size_t row0 = (size_t)b * p.T;
   const size_t zplane = (size_t)p.B * p.T * p.C;
   constexpr int NG = BLOCK_T / 8;                          // 8-column groups of the fragment
@@ -730,13 +492,11 @@ __device__ __forceinline__ void gate_t_epilogue(const FdTapGemm& p, const float*
         for (int s = 0; s < 2; ++s) {
           const int tl = 8 * ci + 2 * q4 + s;              // time step inside the 32-step chunk
           const int t = t0 + 8 * c0 + tl;
-          float yg = acc[4 * (c0 + ci) + s] * p.acc_scale + bg + a_cur[4 * ci + 2 * s];
-          float yf = acc[4 * (c0 + ci) + 2 + s] * p.acc_scale + bf + a_cur[4 * ci + 2 * s + 1];
-          if (t < p.dil) { yg -= lg; yf -= lf; }
-          if (t + p.dil >= p.T) { yg -= hg; yf -= hf; }
+          float g[1] = {acc[4 * (c0 + ci) + s]}, f[1] = {acc[4 * (c0 + ci) + 2 + s]}, z[1];
+          const float add[2][1] = {{a_cur[4 * ci + 2 * s]}, {a_cur[4 * ci + 2 * s + 1]}};
+          fd_epi_gate<1>(p, t, g, f, z, bias, add, lo, hi);
           // scratch [32 steps][8 channels], the two 16-byte halves of a step swapped on every other group of 4 steps
-          sts32(my_scratch + 4u * (tl * 8 + (((e >> 2) ^ ((tl >> 2) & 1)) << 2) + (e & 3)),
-                fd_sigmoid(yg) * fd_tanh(yf));
+          sts32(my_scratch + 4u * (tl * 8 + (((e >> 2) ^ ((tl >> 2) & 1)) << 2) + (e & 3)), z[0]);
         }
       }
     }

@@ -119,13 +119,27 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
 
 // explicit shared-space ld/st (scratch addresses come from integer arithmetic, which would make the compiler fall back
 // to generic LD/ST with their longer latency)
-__device__ __forceinline__ void sts128(uint32_t addr, float x, float y, float z, float w) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
-}
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 r;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(addr) : "memory");
   return r;
+}
+// N (a multiple of 4) consecutive floats: from shared memory, and streaming from global memory (evict-first)
+template <int N>
+__device__ __forceinline__ void lds_f32(uint32_t addr, float (&v)[N]) {
+#pragma unroll
+  for (int q = 0; q < N; q += 4) {
+    const float4 x = lds128(addr + 4u * q);
+    v[q] = x.x; v[q + 1] = x.y; v[q + 2] = x.z; v[q + 3] = x.w;
+  }
+}
+template <int N>
+__device__ __forceinline__ void ldcs_f32(const float* p, float (&v)[N]) {
+#pragma unroll
+  for (int q = 0; q < N; q += 4) {
+    const float4 x = __ldcs(reinterpret_cast<const float4*>(p + q));
+    v[q] = x.x; v[q + 1] = x.y; v[q + 2] = x.z; v[q + 3] = x.w;
+  }
 }
 __device__ __forceinline__ void sts32(uint32_t addr, float x) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(x) : "memory");

@@ -77,6 +77,43 @@ def test_accumulate_and_addend(backend):
     assert rel_l2(out.cpu().numpy(), ref) < 2e-6
 
 
+# every LINEAR operand in one launch, at channel counts that give the wgmma kernel 128-, 32- and 16-column tiles
+@pytest.mark.parametrize("backend", ["simt", "tc"])
+@pytest.mark.parametrize("act", ["relu", "lrelu"])
+@pytest.mark.parametrize("prec", ["f16", "bf16"])
+@pytest.mark.parametrize("Ci,Nn", [(64, 128), (32, 32), (16, 16)])
+def test_linear_all_operands(Ci, Nn, prec, act, backend):
+    B, T, shifts = 3, 203, [-1, 0, 1]
+    pc, bk = N.prec_code(prec), N.backend_code(backend)
+    assert bk != N.BACKEND_TC or N.tc_supported_linear(Nn, Ci, len(shifts))
+    act_code, slope = (N.ACT_RELU, 0.0) if act == "relu" else (N.ACT_LRELU, 0.2)
+    rng = np.random.RandomState(Ci + Nn)
+    d = dev()
+    t32 = lambda *shape: torch.from_numpy(rng.randn(*shape).astype(np.float32)).to(d)
+    a, w = t32(B, T, Ci), t32(Nn, 3 * Ci) / np.sqrt(3 * Ci)
+    bias, add, res, resp, prev = t32(B, Nn), t32(B, T, Nn), t32(B, T, Nn), t32(B, T, Nn), t32(B, T, Nn)
+    mask = torch.zeros((B, T), dtype=torch.uint8, device=d)
+    mask[1, T // 3:] = 1
+    mask[2, ::7] = 1
+    ap, rp, s = N.split_nwc(a, pc), N.split_nwc(resp, pc), N.pow2_scale(w)
+    wp = N.pack_weight(w, pc, s)
+    out = prev.clone()
+    outp = torch.zeros((2, B, T, Nn), dtype=torch.int16, device=d)
+    N.gemm_cl(ap, Ci, wp, Nn, 3 * Ci, B, T, [(0, sh, 0, Ci) for sh in shifts], bias=bias, bias_per_item=True,
+              addend=add, res_f32=res, res_planes=rp, res_scale=0.75, row_mask=mask, out_f32=out, out_planes=outp,
+              w_inv_scale=1.0 / s, post_scale=0.5, planes_scale=2.0, act=act_code, act_slope=slope, out_accum=True,
+              prec=pc, backend=bk)
+    torch.cuda.synchronize()
+    f64 = lambda x: x.cpu().numpy().astype(np.float64)
+    y = (tap_gemm_ref(planes_to_f64(ap, pc), planes_to_f64(wp, pc) / s, shifts) + f64(bias)[:, None, :] + f64(add)
+         + f64(res) + 0.75 * planes_to_f64(rp, pc)) * 0.5 + f64(prev)
+    y[mask.cpu().numpy().astype(bool)] = 0
+    got = out.cpu().numpy()
+    assert rel_l2(got, y) < (2e-6 if prec == "f16" else 5e-5), (rel_l2(got, y), np.abs(got - y).max())
+    pl = np.where(y > 0, 2.0 * y, 2.0 * slope * y)
+    assert rel_l2(planes_to_f64(outp, pc), pl) < (2e-6 if prec == "f16" else 2e-5)
+
+
 def test_tc_matches_simt_full_width_block():
     """One WaveNet residual block at the real width (C=512, E=256), wgmma vs SIMT twin on identical planes."""
     import math
