@@ -102,7 +102,6 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sm
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory"); }
 
 // One conv of the pair over the whole tile: acc[j] (block j of this warpgroup) += A(shifted rows) x W for every listed
 // weight unit.  A comes from the swizzled activation tile at a_base (a_kb bytes per 64-channel block, a_plane bytes
@@ -277,7 +276,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
     // ---- epilogue 1: bias, LeakyReLU, zero outside [0,T), split planes -> mid tile (c2's A operand).  The mid tile is
     //      also the staging image of the previous tile's output: its TMA stores must have read it.
     if (issuer) bulk_wait_read0();
-    consumer_sync();
+    named_bar_sync<1, FD_TC_CONSUMER_THREADS>();
 #pragma unroll
     for (int j = 0; j < K::BPW; ++j) {
 #pragma unroll
@@ -325,13 +324,13 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(in_empty);            // this warp is done with the input tile
-    consumer_sync();                                 // the whole mid tile is written
+    named_bar_sync<1, FD_TC_CONSUMER_THREADS>();     // the whole mid tile is written
 
     // ---- GEMM2: output rows r, mid rows r + tap
     rp_gemm<C, PREC>(acc, p, p.n2, p.ul2, p.km2, p.masked2 != 0, mid_u, K::MID_KB_BYTES, K::MID_PLANE_BYTES, 1,
                      blk0 * 64 + 16 * wq, w_u, STAGE_BYTES_RT, ring, lane);
     wg_fence_operand(acc);
-    consumer_sync();                                 // every warpgroup is done reading the mid tile
+    named_bar_sync<1, FD_TC_CONSUMER_THREADS>();     // every warpgroup is done reading the mid tile
 
     // ---- epilogue 2: lrelu(acc * inv_s2) * planes_scale -> split planes -> staging image (mid tile) -> TMA stores
 #pragma unroll
@@ -354,7 +353,7 @@ fd_respair_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_con
       }
     }
     fence_async_smem();
-    consumer_sync();
+    named_bar_sync<1, FD_TC_CONSUMER_THREADS>();
     if (issuer) {
       for (int j = 0; j < K::ROWS / 128; ++j) {
         const CUtensorMap* tm = j == K::ROWS / 128 - 1 ? &tm_out_last : &tm_out;

@@ -282,9 +282,9 @@ fd_tapgemm_tc_kernel(const __grid_constant__ CUtensorMap tm_src0, const __grid_c
     // columns / item -- with a single column tile that is once per launch
     if (EPI == FD_EPI_LINEAR && bias_key<EPI>(p, b, n0) != staged_key) {
       staged_key = bias_key<EPI>(p, b, n0);
-      asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory");
+      named_bar_sync<1, FD_TC_CONSUMER_THREADS>();
       stage_bias<BLOCK_N, EPI>(p, b, n0, bias_s, threadIdx.x, FD_TC_CONSUMER_THREADS);
-      asm volatile("bar.sync 1, %0;" ::"r"(FD_TC_CONSUMER_THREADS) : "memory");
+      named_bar_sync<1, FD_TC_CONSUMER_THREADS>();
     }
 
     // ---- mainloop: 16 elements * 2 B along K inside the swizzle row per k16 step
