@@ -1,13 +1,14 @@
 """fish_diffusion_b200 -- H100-native (sm_90a) implementation of fish-diffusion's data-parallel hot path:
-the WaveNet diffusion denoiser + DDPM/PLMS/UniPC samplers and the NSF-HiFiGAN vocoder with its mel front end,
+the WaveNet and ConvNext diffusion denoisers + DDPM/PLMS/UniPC samplers and the NSF-HiFiGAN vocoder with its mel front end,
 behind the reference's DENOISERS / DIFFUSIONS / VOCODERS registries.  See DESIGN.md and INTEGRATION.md.
 
 Importing this package registers the native classes under the reference's registry names
-("WaveNetDenoiser", "GaussianDiffusion", "NsfHifiGAN").  The compute path is libfishdiff_b200.so
+("WaveNetDenoiser", "ConvNextDenoiser", "GaussianDiffusion", "NsfHifiGAN").  The compute path is libfishdiff_b200.so
 (hand-written CUDA for sm_90a, C ABI in include/fishdiff_b200.h); there is no CPU or PyTorch fallback.
 """
 from .registry import DENOISERS, DIFFUSIONS, VOCODERS, Registry  # noqa: F401
 from .wavenet import WaveNet  # noqa: F401
+from .convnext import ConvNext  # noqa: F401
 from .diffusion import GaussianDiffusion, NaiveNoisePredictor, PLMSNoisePredictor, UNIPCNoisePredictor  # noqa: F401
 from .nsf_hifigan import Generator, NsfHifiGAN  # noqa: F401
 from .mel import (MelSpectrogram, PitchAdjustableMelSpectrogram, dynamic_range_compression, get_mel_from_audio,  # noqa: F401

@@ -19,8 +19,8 @@ LIB_PATH = os.environ.get("FISHDIFF_B200_LIB") or os.path.join(_HERE, "libfishdi
 PREC_F16, PREC_BF16 = 0, 1
 PREC_SINGLE = 0x10   # or-ed into the prec of GEMM calls: one product over the hi planes
 BACKEND_TC, BACKEND_SIMT = 0, 1
-ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
-ABI_VERSION = 3
+ACT_NONE, ACT_RELU, ACT_LRELU, ACT_GELU = 0, 1, 2, 3
+ABI_VERSION = 4
 
 
 class NativeError(RuntimeError):
@@ -86,6 +86,29 @@ class WaveNetFwdDesc(ctypes.Structure):
     ]
 
 
+class ConvNextFwdDesc(ctypes.Structure):
+    """struct fd_convnext_fwd_desc (include/fishdiff_b200.h)."""
+    _fields_ = [
+        ("x_planes", c_void_p), ("cond_planes", c_void_p), ("steps", c_void_p), ("x_mask", c_void_p),
+        ("cond_mask", c_void_p), ("out", c_void_p),
+        ("w_in", c_void_p), ("b_in", c_void_p), ("w_in_inv", c_float),
+        ("emb_w0", c_void_p), ("emb_b0", c_void_p), ("emb_w1", c_void_p), ("emb_b1", c_void_p),
+        ("w_step", c_void_p), ("b_step", c_void_p),
+        ("w_c1", c_void_p), ("b_c1", c_void_p), ("w_c1_inv", c_float),
+        ("w_c2", c_void_p), ("b_c2", c_void_p), ("w_c2_inv", c_float),
+        ("w_cp", c_void_p), ("dw_w", c_void_p), ("dw_b", c_void_p), ("ln_w", c_void_p), ("ln_b", c_void_p),
+        ("w_pw1", c_void_p), ("b_pw1", c_void_p), ("w_pw2", c_void_p), ("b_pw2", c_void_p),
+        ("w_o1", c_void_p), ("b_o1", c_void_p), ("w_o1_inv", c_float),
+        ("w_o2", c_void_p), ("b_o2", c_void_p), ("w_o2_inv", c_float),
+        ("w_cp_inv", c_float * 64), ("w_pw1_inv", c_float * 64), ("w_pw2_inv", c_float * 64), ("dilation", c_int * 64),
+        ("xr", c_void_p), ("a", c_void_p), ("h", c_void_p), ("cpl", c_void_p), ("p", c_void_p),
+        ("s", c_void_p), ("sv", c_void_p), ("mlp_ws", c_void_p),
+        ("B", c_int), ("T", c_int), ("M", c_int), ("C", c_int), ("H", c_int), ("E", c_int), ("L", c_int), ("Bs", c_int),
+        ("prec", c_int), ("backend", c_int),
+        ("cond_proj", c_void_p),
+    ]
+
+
 class WaveNetBwdDesc(ctypes.Structure):
     """struct fd_wavenet_bwd_desc (include/fishdiff_b200.h)."""
     _fields_ = [
@@ -143,6 +166,9 @@ _SIGS = {
                              [c_float, c_float, c_int, c_int, c_int, c_void_p]),
     "fd_wavenet_fwd": (c_int, [POINTER(WaveNetFwdDesc), c_void_p]),
     "fd_wavenet_cond_proj": (c_int, [POINTER(WaveNetFwdDesc), c_void_p]),
+    "fd_convnext_dwln_fwd": (c_int, [c_void_p] * 3 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p]),
+    "fd_convnext_fwd": (c_int, [POINTER(ConvNextFwdDesc), c_void_p]),
+    "fd_convnext_cond_proj": (c_int, [POINTER(ConvNextFwdDesc), c_void_p]),
     "fd_conv_cl_fwd": (c_int, [POINTER(ConvDesc), c_void_p]),
     "fd_respair_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "fd_respair_fwd": (c_int, [POINTER(ResPairDesc), c_void_p]),

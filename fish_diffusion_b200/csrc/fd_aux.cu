@@ -217,7 +217,7 @@ __global__ void k_step_embed(const float* __restrict__ steps, float* __restrict_
 }
 
 // y[bs][n] = act( sum_k x[bs][k] * w[n*w_pitch + k] + bias[n] ), one warp per n, all bs.
-// act: 0 none, 1 Mish (x * tanh(softplus(x)), softplus threshold 20 as in torch)
+// act: 0 none, 1 Mish (x * tanh(softplus(x)), softplus threshold 20 as in torch), 2 exact GELU
 __global__ void k_small_linear(const float* __restrict__ x, const float* __restrict__ w,
                                const float* __restrict__ bias, float* __restrict__ y, int Bs, int K, int N,
                                long long w_pitch, int act) {
@@ -236,6 +236,8 @@ __global__ void k_small_linear(const float* __restrict__ x, const float* __restr
       if (act == 1) {
         const float sp = v > 20.f ? v : log1pf(expf(v));
         v = v * tanhf(sp);
+      } else if (act == 2) {
+        v = fd_gelu(v);
       }
       y[(size_t)bs * N + warp] = v;
     }
@@ -383,6 +385,25 @@ inline int grid_for(long long work, int block = 256, int cap = 132 * 16) {
 
 }  // namespace
 
+int fd_small_linear(const float* x, const float* w, const float* bias, float* y, int Bs, int K, int N, long long w_pitch,
+                    int act, cudaStream_t st) {
+  k_small_linear<<<(unsigned)(((long long)N * 32 + 255) / 256), 256, 0, st>>>(x, w, bias, y, Bs, K, N, w_pitch, act);
+  FD_LAUNCHED();
+  return 0;
+}
+
+int fd_step_mlp(const float* steps, const float* w0, const float* b0, const float* w1, const float* b1, float* s_out,
+                float* ws, int Bs, int C, int H, int act, cudaStream_t st) {
+  FD_REQUIRE(C % 2 == 0 && C >= 4 && H > 0, "step mlp: bad C=%d H=%d", C, H);
+  float* emb = ws;                 // [Bs][C]
+  float* h = ws + (size_t)Bs * C;  // [Bs][H]
+  k_step_embed<<<grid_for((long long)Bs * C / 2), 256, 0, st>>>(steps, emb, Bs, C);
+  FD_LAUNCHED();
+  int rc = fd_small_linear(emb, w0, b0, h, Bs, C, H, C, act, st);
+  if (rc) return rc;
+  return fd_small_linear(h, w1, b1, s_out, Bs, H, C, H, 0, st);
+}
+
 extern "C" {
 
 int fd_split_ncw(const float* src, const uint8_t* mask, uint16_t* planes, int B, int C, int T, int prec,
@@ -460,17 +481,7 @@ int fd_wavenet_pack_layers(const float* const* conv_w, const float* const* cond_
 int fd_wavenet_step_mlp(const float* steps, const float* w0, const float* b0, const float* w1, const float* b1,
                         float* s_out, float* ws, int Bs, int C, void* stream) {
   FD_DEVICE_GUARD();
-  FD_REQUIRE(C % 2 == 0 && C >= 4, "fd_wavenet_step_mlp: bad C=%d", C);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* emb = ws;                 // [Bs][C]
-  float* h = ws + (size_t)Bs * C;  // [Bs][4C]
-  k_step_embed<<<grid_for((long long)Bs * C / 2), 256, 0, st>>>(steps, emb, Bs, C);
-  FD_LAUNCHED();
-  k_small_linear<<<(4 * C * 32 + 255) / 256, 256, 0, st>>>(emb, w0, b0, h, Bs, C, 4 * C, C, 1);
-  FD_LAUNCHED();
-  k_small_linear<<<(C * 32 + 255) / 256, 256, 0, st>>>(h, w1, b1, s_out, Bs, 4 * C, C, 4 * C, 0);
-  FD_LAUNCHED();
-  return 0;
+  return fd_step_mlp(steps, w0, b0, w1, b1, s_out, ws, Bs, C, 4 * C, 1, (cudaStream_t)stream);
 }
 
 int fd_wavenet_gate_bias(const float* s, const float* wd, const float* bd, const float* w1p, const float* bias_sum,
@@ -479,8 +490,8 @@ int fd_wavenet_gate_bias(const float* s, const float* wd, const float* bd, const
   FD_DEVICE_GUARD();
   cudaStream_t st = (cudaStream_t)stream;
   // d[bs][l][c] = Wd[l][c][:] . s[bs] + bd[l][c]
-  k_small_linear<<<(L * C * 32 + 255) / 256, 256, 0, st>>>(s, wd, bd, ws, Bs, C, L * C, C, 0);
-  FD_LAUNCHED();
+  int rc = fd_small_linear(s, wd, bd, ws, Bs, C, L * C, C, 0, st);
+  if (rc) return rc;
   const long long warps = (long long)L * Bs * 2 * C;
   k_gate_bias<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(ws, w1p, bias_sum, gb_full, gb_lo, gb_hi, L, Bs,
                                                                    C, KT);

@@ -31,6 +31,7 @@
 #define FD_ACT_NONE 0
 #define FD_ACT_RELU 1
 #define FD_ACT_LRELU 2
+#define FD_ACT_GELU 3
 
 struct FdSeg {
   int src;    // which source tensor (0/1)
@@ -62,7 +63,7 @@ struct FdTapGemm {
 
   // ---- FD_EPI_LINEAR:  y = acc*acc_scale + bias[n] + addend[b,t,n] + res[b,t,n];  y *= post_scale
   //      if out_f32:   v = accum ? out_f32 + y : y ;  out_f32 = v   (else v = y)
-  //      if out_planes: planes = split(act(v * planes_scale))
+  //      if out_planes: planes = split(act(v * planes_scale)), act = none / relu / leaky-relu / exact GELU
   //      rows with row_mask[b,t] != 0 produce zeros.
   const float* bias;        // [n_total] or per item [B][n_total] with bias_bstride
   int bias_bstride;
@@ -179,6 +180,9 @@ __device__ __forceinline__ void fd_combine2(uint32_t hi2, uint32_t lo2, int prec
 
 // branch-free activation of the linear epilogue: slope = 1 (none), 0 (ReLU) or the LeakyReLU slope
 __device__ __forceinline__ float fd_act(float w, float slope) { return fmaf(slope, fminf(w, 0.f), fmaxf(w, 0.f)); }
+
+// exact GELU (torch's nn.GELU() / F.gelu default, approximate="none"): 0.5 x (1 + erf(x / sqrt 2)), erff, no tanh form
+__device__ __forceinline__ float fd_gelu(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 
 // accurate-enough transcendental pieces (relative error ~1e-7; tanh.approx is 1e-3 and is NOT used)
 __device__ __forceinline__ float fd_sigmoid(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
@@ -370,8 +374,13 @@ __device__ __forceinline__ void fd_epi_linear(const FdTapGemm& p, const FdRows<I
     if (p.out_f32 != nullptr) fd_store_f32<V>(p.out_f32 + off[r], a[r]);
     if (p.out_planes != nullptr) {
       float v[V];
+      if (p.act == FD_ACT_GELU) {   // uniform over the launch; the slope path below stays as it was
 #pragma unroll
-      for (int i = 0; i < V; ++i) v[i] = fd_act(a[r][i] * p.planes_scale, slope);
+        for (int i = 0; i < V; ++i) v[i] = fd_gelu(a[r][i] * p.planes_scale);
+      } else {
+#pragma unroll
+        for (int i = 0; i < V; ++i) v[i] = fd_act(a[r][i] * p.planes_scale, slope);
+      }
       fd_store_planes<V>(p.out_planes, plane, off[r], v, prec);
     }
   }

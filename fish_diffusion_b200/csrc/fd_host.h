@@ -33,3 +33,11 @@ struct FdDeviceGuard {
 constexpr int FD_MAX_DEVICES = 64;
 int fd_current_device();          // cudaGetDevice (clamped to [0, FD_MAX_DEVICES))
 int fd_device_sms(int dev);       // multiprocessor count, cached
+
+// the step-vector kernels of fd_aux.cu, shared by the WaveNet and ConvNext forwards:
+//   y[bs][n] = act(w[n * w_pitch + :] . x[bs] + bias[n])  (act 0 none, 1 Mish, 2 exact GELU; bias may be NULL)
+int fd_small_linear(const float* x, const float* w, const float* bias, float* y, int Bs, int K, int N, long long w_pitch,
+                    int act, cudaStream_t st);
+//   s_out[Bs][C] = w1 . act(w0 . DiffusionEmbedding(steps) + b0) + b1,  w0 [H][C], w1 [C][H]; ws: Bs * (C + H) floats
+int fd_step_mlp(const float* steps, const float* w0, const float* b0, const float* w1, const float* b1, float* s_out,
+                float* ws, int Bs, int C, int H, int act, cudaStream_t st);

@@ -43,12 +43,13 @@ to_torch = partial(torch.tensor, dtype=torch.float32)
 
 def hoist_cond_proj(denoiser, B: int, T: int, device) -> bool:
     """Whether a sampler call keeps the conditioner projection of all layers resident and computes it once instead of
-    inside every GEMM1 launch.  Only with three tensor-core products: there the projection is a seventh of GEMM1's MMA
-    work; single-product GEMM1 gains less than the fp32 projection costs to read (at B=32, T=4000 the f16x1 sampler ran
-    3.34 s hoisted against 3.23 s fused, DESIGN.md section 5).  And only when the buffer takes at most a quarter of the
-    card's total memory (not of the free memory, which other processes on a shared GPU change from run to run), so a
-    given shape takes the same path every time."""
-    if N.mma_code(denoiser.precision) & N.PREC_SINGLE:
+    inside every evaluation.  A denoiser that can fuse the projection into its GEMMs (`fuses_cond_proj`, the WaveNet's
+    GEMM1) hoists it only with three tensor-core products: there the projection is a seventh of GEMM1's MMA work;
+    single-product GEMM1 gains less than the fp32 projection costs to read (at B=32, T=4000 the f16x1 sampler ran
+    3.34 s hoisted against 3.23 s fused, DESIGN.md section 5).  Every denoiser hoists only when the buffer takes at most
+    a quarter of the card's total memory (not of the free memory, which other processes on a shared GPU change from run
+    to run), so a given shape takes the same path every time."""
+    if getattr(denoiser, "fuses_cond_proj", False) and N.mma_code(denoiser.precision) & N.PREC_SINGLE:
         return False
     nbytes = 4 * int(np.prod(denoiser.cond_proj_shape(B, T)))
     return nbytes <= torch.cuda.mem_get_info(device)[1] // 4
@@ -378,7 +379,7 @@ class GaussianDiffusion(nn.Module):
             shape = den.cond_proj_shape(B, T)
             if ws.get("cond_proj") is None or tuple(ws["cond_proj"].shape) != shape:
                 ws["cond_proj"] = torch.empty(shape, dtype=torch.float32, device=dev)
-            cond_proj = den.cond_projection(cond_planes, ws["cond_proj"])
+            cond_proj = den.cond_projection(cond_planes, ws["cond_proj"], cond_mask=cmask)
         else:
             ws["cond_proj"] = None
         if original_mel is None:
@@ -415,8 +416,10 @@ class GaussianDiffusion(nn.Module):
             steps = step_table.get(t_float)
             if steps is None:
                 steps = step_table[t_float] = torch.tensor([t_float], dtype=torch.float32, device=dev)
+            # the conditioner mask goes to every evaluation, the PLMS look-ahead's included: the planes were split with
+            # it once for the whole call, and a hoisted projection was computed with it
             return den.forward_cl(xp, steps, cond_planes, x_mask=x_masks if masks else None, out=out,
-                                  cond_proj=cond_proj)
+                                  cond_proj=cond_proj, cond_mask=cmask)
 
         if noise_predictor in ("naive", "plms") and len(chunks) > 1:   # one upload for the whole schedule
             tab = torch.tensor([float(t) for t in chunks], dtype=torch.float32, device=dev)

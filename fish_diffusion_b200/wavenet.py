@@ -19,6 +19,7 @@ import torch
 from torch import nn
 
 from . import _native as N
+from .graphs import run_cached
 from .registry import DENOISERS
 
 
@@ -87,6 +88,9 @@ class WaveNet(nn.Module):
         "bf16x1" keep that storage but multiply the hi planes only (one tensor-core product, half-precision operands)
       backend:   "auto" (wgmma when the shape has a tensor-core instantiation, else the SIMT twin), "tc", "simt"
     """
+
+    # GEMM1 can run the conditioner projection in its own K loop (see diffusion.hoist_cond_proj)
+    fuses_cond_proj = True
 
     def __init__(self, mel_channels=128, d_encoder=256, residual_channels=512, residual_layers=20,
                  use_linear_bias=False, dilation_cycle=None, precision="f16", backend="auto"):
@@ -336,12 +340,13 @@ class WaveNet(nn.Module):
         return (self.n_layers, B, T, 2 * self.residual_channels)
 
     @torch.no_grad()
-    def cond_projection(self, cond_planes, out):
+    def cond_projection(self, cond_planes, out, cond_mask=None):
         """Every layer's conditioner_projection(conditioner) (wavenet.py:108) without its bias, for cond_planes
         [2,B,T,E], into the caller-owned fp32 buffer `out` (cond_proj_shape) in W1's packed column order: L linear
         tap-GEMMs over the conditioner columns of the current weight pack (fd_wavenet_cond_proj).  forward_cl(...,
         cond_proj=out) then skips those columns in GEMM1; a sampler computes it once per call, since all its
-        evaluations share the conditioner.  Returns `out`."""
+        evaluations share the conditioner.  cond_mask is accepted for the sampler protocol and not used: the WaveNet
+        masks the raw conditioner (wavenet.py:219-221), which the caller's cond_planes already are.  Returns `out`."""
         dev = cond_planes.device
         N.require_cuda(cond_planes, "cond_planes")
         _, B, T, E = cond_planes.shape
@@ -361,12 +366,13 @@ class WaveNet(nn.Module):
         return out
 
     @torch.no_grad()
-    def forward_cl(self, x_planes, steps, cond_planes, x_mask=None, out=None, cond_proj=None):
+    def forward_cl(self, x_planes, steps, cond_planes, x_mask=None, out=None, cond_proj=None, cond_mask=None):
         """Channels-last entry used by the fused sampler.
 
         x_planes [2,B,T,M] int16 split planes, steps float32 [1] or [B] (device), cond_planes [2,B,T,E],
         x_mask uint8/bool [B,T] or None (True = masked).  cond_proj: what cond_projection made of these cond_planes
-        under the current weights, or None (GEMM1 then projects the conditioner itself).  Returns eps fp32 [B,T,M]."""
+        under the current weights, or None (GEMM1 then projects the conditioner itself).  cond_mask: ignored, as in
+        cond_projection.  Returns eps fp32 [B,T,M]."""
         dev = x_planes.device
         N.require_cuda(x_planes, "x_planes")
         _, B, T, M = x_planes.shape
@@ -379,51 +385,25 @@ class WaveNet(nn.Module):
         if Bs not in (1, B):
             raise ValueError(f"diffusion_step must have 1 or B={B} entries, got {Bs}")
         ws = self._workspace(dev, B, T, Bs)
-        st = N.stream_ptr(dev)
         lib = N.lib()
         if x_mask is not None:
             x_mask = x_mask.to(device=dev, dtype=torch.uint8).contiguous()
         if out is None:
             out = torch.empty((B, T, M), dtype=torch.float32, device=dev)
 
-        # ONE native call per evaluation (fd_wavenet_fwd issues the ~45 launches back to back); when the same buffers
-        # come back (the sampler loop) the call is captured into a CUDA graph on its second use and replayed afterwards,
-        # which also removes the per-launch tensor-map encodes from the host path.
+        # ONE native call per evaluation (fd_wavenet_fwd issues the ~45 launches back to back), replayed from a CUDA
+        # graph when the same buffers come back (the sampler loop)
         steps_buf = ws["steps"]
         steps_buf.copy_(steps, non_blocking=True)
         if cond_proj is not None and tuple(cond_proj.shape) != self.cond_proj_shape(B, T):
             raise ValueError(f"cond_proj must have shape {self.cond_proj_shape(B, T)}")
         d = self._fwd_desc(pk, ws, x_planes, cond_planes, steps_buf, x_mask, out, B, T, Bs)
         d.cond_proj = N.ptr(cond_proj)
-        use_graph = self.use_graph and not N.prof_is_on()
-        if not use_graph:
-            N.check(lib.fd_wavenet_fwd(ctypes.byref(d), st), "fd_wavenet_fwd")
-            return out
         key = (x_planes.data_ptr(), cond_planes.data_ptr(), out.data_ptr(), 0 if x_mask is None else x_mask.data_ptr(),
                0 if cond_proj is None else cond_proj.data_ptr(), B, T, Bs, self._pack_key, id(ws))
-        ent = self._graphs.get(key)
-        if ent is None:                      # first sight of these buffers: run eagerly (lazy inits happen here)
-            if len(self._graphs) >= 4:
-                self._graphs.clear()
-            self._graphs[key] = {"graph": None, "keep": (x_planes, cond_planes, out, x_mask, cond_proj, pk)}
-            N.check(lib.fd_wavenet_fwd(ctypes.byref(d), st), "fd_wavenet_fwd")
-            return out
-        if ent["graph"] is None:
-            # capture on a side stream without torch.cuda.graph()'s device synchronise + empty_cache (the call sits in
-            # the middle of a sampler loop); nothing inside allocates
-            g = torch.cuda.CUDAGraph()
-            cur = torch.cuda.current_stream(dev)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                g.capture_begin()
-                try:
-                    N.check(lib.fd_wavenet_fwd(ctypes.byref(d), N.stream_ptr(dev)), "fd_wavenet_fwd")
-                finally:
-                    g.capture_end()
-            cur.wait_stream(side)
-            ent["graph"] = g
-        ent["graph"].replay()
+        run_cached(self._graphs, key, (x_planes, cond_planes, out, x_mask, cond_proj, pk),
+                   lambda: N.check(lib.fd_wavenet_fwd(ctypes.byref(d), N.stream_ptr(dev)), "fd_wavenet_fwd"), dev,
+                   self.use_graph)
         return out
 
     def _fwd_desc(self, pk, ws, x_planes, cond_planes, steps, x_mask, out, B, T, Bs):

@@ -32,7 +32,7 @@ extern "C" {
 #define FD_PREC_SINGLE 0x10
 #define FD_BACKEND_TC 0
 #define FD_BACKEND_SIMT 1
-#define FD_ABI_VERSION 3
+#define FD_ABI_VERSION 4
 
 /* ------------------------------------------------------------------------------------------- misc */
 int fd_abi_version(void);
@@ -138,6 +138,65 @@ int fd_wavenet_fwd(const fd_wavenet_fwd_desc* d, void* stream);
  * B*T*2C must stay below 2^32. */
 int fd_wavenet_cond_proj(const fd_wavenet_fwd_desc* d, void* stream);
 
+/* ------------------------------------------------------------------------- ConvNext denoiser */
+/* Front of one ConvNeXtBlock (convnext.py:64-78) as one kernel:
+ *   u[b,t,c]   = mask[b,t] ? 0 : x[b,t,c] + step[b][c] + cond_proj[b,t,c]      (zero outside 0 <= t < T)
+ *   v[b,t,c]   = dw_b[c] + sum_{j<7} dw_w[c][j] u[b, t + (j - 3) dilation, c]
+ *   out[b,t,:] = LayerNorm(v[b,t,:]) over the C channels (eps 1e-6, biased variance, affine ln_w / ln_b)
+ * x_planes / out_planes [2][B][T][C] split planes; cond_proj fp32 [B][T][C] (one layer's slice of the buffer
+ * fd_convnext_cond_proj fills, or a one-layer scratch); step: item b's vector at step + b * step_bstride (0 = one
+ * vector for the batch; a multiple of 4); x_mask [B][T] or NULL; dw_w [C][7], dw_b / ln_w / ln_b [C].  u is staged in
+ * shared memory only.  C a multiple of 16, at most 1024; any dilation >= 1; 64-bit offsets. */
+int fd_convnext_dwln_fwd(const uint16_t* x_planes, const float* cond_proj, const float* step, long long step_bstride,
+                         const uint8_t* x_mask, const float* dw_w, const float* dw_b, const float* ln_w,
+                         const float* ln_b, uint16_t* out_planes, int B, int T, int C, int dilation, int prec,
+                         void* stream);
+/* One complete ConvNext.forward (convnext.py:208-261, cross_attention=False) on channels-last split planes as ONE native
+ * call, capturable into a CUDA graph (nothing synchronises or allocates):
+ *   step vectors  sv[Bs][L*C] = Wstep . (emb_w1 . gelu(emb_w0 . DiffusionEmbedding(steps) + emb_b0) + emb_b1) + b_step
+ *   head          xr = mask(gelu(W_in x + b_in))
+ *   L blocks      a = dwln(xr, cond_proj[l], sv[:, l]) ; h = gelu(W_pw1[l] a + b_pw1[l]) ;
+ *                 xr = mask(xr + W_pw2[l] h + b_pw2[l])   (gamma folded into W_pw2 / b_pw2; in place)
+ *   tail          out = mask(W_o2 gelu(W_o1 xr + b_o1) + b_o2)
+ * Weights: packed split planes [2][N][K] (stacks [L][2][N][K]) prescaled by 1 / *_inv, fp32 vectors; w_step [L*C][C]
+ * stacks the diffusion_step_projections, b_step [L*C] their biases plus the condition_projection biases.
+ * cond_proj: fp32 [L][B][T][C] filled by fd_convnext_cond_proj for these cond planes and weights, or NULL: the call then
+ * runs the conditioner MLP into cpl and each layer's condition projection into the p scratch itself. */
+typedef struct fd_convnext_fwd_desc {
+  const uint16_t* x_planes;     /* [2][B][T][M] */
+  const uint16_t* cond_planes;  /* [2][B][T][E] */
+  const float* steps;           /* [Bs] diffusion steps (float), Bs = 1 or B */
+  const uint8_t* x_mask;        /* [B][T] or NULL (convnext.py:236-237, 70-71, 86-87, 257-258) */
+  const uint8_t* cond_mask;     /* [B][T] or NULL: masks the conditioner MLP's output (convnext.py:239-240) */
+  float* out;                   /* eps fp32 [B][T][M] */
+  const uint16_t* w_in; const float* b_in; float w_in_inv;                 /* [2][C][M] */
+  const float* emb_w0; const float* emb_b0; const float* emb_w1; const float* emb_b1;   /* [H][C], [H], [C][H], [C] */
+  const float* w_step; const float* b_step;                                /* [L*C][C], [L*C] */
+  const uint16_t* w_c1; const float* b_c1; float w_c1_inv;                 /* [2][H][E] */
+  const uint16_t* w_c2; const float* b_c2; float w_c2_inv;                 /* [2][C][H] */
+  const uint16_t* w_cp;                                                    /* [L][2][C][C] */
+  const float* dw_w; const float* dw_b; const float* ln_w; const float* ln_b;  /* [L][C][7], [L][C] x 3 */
+  const uint16_t* w_pw1; const float* b_pw1;                               /* [L][2][H][C], [L][H] */
+  const uint16_t* w_pw2; const float* b_pw2;                               /* [L][2][C][H], [L][C] */
+  const uint16_t* w_o1; const float* b_o1; float w_o1_inv;                 /* [2][C][C] */
+  const uint16_t* w_o2; const float* b_o2; float w_o2_inv;                 /* [2][M][C] */
+  float w_cp_inv[64], w_pw1_inv[64], w_pw2_inv[64];
+  int dilation[64];
+  /* workspace (caller-owned, see ConvNext._workspace): planes xr / a [2][B][T][C], h [2][B][T][H], cpl [2][B][T][C]
+   * (cond MLP output; unused by fd_convnext_fwd when cond_proj is set), p fp32 [B][T][C] (likewise), s [Bs][C],
+   * sv [Bs][L*C], mlp_ws Bs*(C+H) floats */
+  uint16_t* xr; uint16_t* a; uint16_t* h; uint16_t* cpl; float* p;
+  float* s; float* sv; float* mlp_ws;
+  int B, T, M, C, H, E, L, Bs;
+  int prec, backend;            /* prec may carry FD_PREC_SINGLE (GEMMs only) */
+  float* cond_proj;
+} fd_convnext_fwd_desc;
+int fd_convnext_fwd(const fd_convnext_fwd_desc* d, void* stream);
+/* Fills d->cond_proj [L][B][T][C] from d->cond_planes: the conditioner MLP (convnext.py:177-181, 234) masked by
+ * cond_mask into cpl (h as its hidden workspace), then every layer's condition_projection without bias.  Uses
+ * cond_planes, cond_mask, w_c1, b_c1, w_c2, b_c2, w_cp and their scales, cpl, h, B, T, C, H, E, L, prec, backend. */
+int fd_convnext_cond_proj(const fd_convnext_fwd_desc* d, void* stream);
+
 /* One ResidualBlock.forward (wavenet.py:106-120), fused as two tap-GEMM launches:
  *   GEMM1  y = [W_conv(3 taps) | W_cond] . [x(t-d), x(t), x(t+d), cond(t)] + gate bias ; z = sigmoid(y_g)*tanh(y_f)
  *   GEMM2  o = W_out z + b ;  x <- (x + o_res)/sqrt(2) (in place) ;  skip_acc (+)= o_skip
@@ -173,7 +232,8 @@ typedef struct fd_conv_desc {
   int shifts[16];
   float w_inv_scale, post_scale, planes_scale, act_slope;
   int out_accum;             /* out_f32 += */
-  int act;                   /* 0 none, 1 relu, 2 leaky-relu(act_slope): applied to the planes output only */
+  int act;                   /* 0 none, 1 relu, 2 leaky-relu(act_slope), 3 exact GELU 0.5 x (1 + erf(x / sqrt 2)):
+                                applied to the planes output only */
   int prec, backend;
 } fd_conv_desc;
 int fd_conv_cl_fwd(const fd_conv_desc* d, void* stream);
@@ -308,7 +368,7 @@ typedef struct fd_gemm_desc {
   float* out_f32;
   uint16_t* out_planes;
   float w_inv_scale, res_scale, post_scale, planes_scale, act_slope;
-  int out_accum, act, prec, backend;
+  int out_accum, act, prec, backend;   /* act as in fd_conv_desc (3 = exact GELU) */
   int bias_bstride;   /* 0: bias [n_total]; n_total: one bias vector per batch item, bias [B][n_total] (per-utterance
                          speaker / pitch-shift embeddings of DiffSinger.forward_features, diffsinger.py:95-121) */
   /* gate backward fused into the epilogue (training, either back end): when gate_y != NULL the accumulator is
